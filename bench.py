@@ -2,6 +2,7 @@
 """bench.py — the hot-path benchmark (driver contract).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|...]
+                    [--dump-outputs DIR]
 
 One "step" = one CSR SpMM (sum) pass over the synthetic matrix of BASELINE.json configs[1]:
 1M x 1M (per GPU), ~16 nnz/row, dense operand F=128 bf16 (SURVEY §8d generator G2 / G5).
@@ -11,6 +12,7 @@ H2D/D2H inside the timed region); `roofline` = algorithmic HBM bytes / step time
 peak; `cpu_baseline` = the reference's own CPU spmm (oracle/_ref) on this box's host cores.
 
 `--impl reference` times the reference's CPU operator itself on the same config (rank 0 only).
+`--dump-outputs DIR` writes a fixed, seeded row sample of what the last timed step returned (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -293,6 +295,22 @@ def _spmm_parity(oracle, rowptr_h, col_h, value_h, x_h, out_rows, rows, rel):
     return bool((err <= rel * bound + 1e-30).all()), float((err / bound.clamp_min(1e-30)).max())
 
 
+def dump_outputs(out_dir, out, rank, world):
+    """Write a fixed, seeded sample of the rows the timed path returned in its last step: DIR/spmm_out_rank<r>.npy
+    (float32 [rows, F]) and the sampled row numbers, DIR/spmm_out_rows_rank<r>.npy (float64). At most 32 MB of
+    values over all ranks. The inputs are generated from fixed seeds, so two builds run with the same arguments can be
+    compared output for output."""
+    import numpy as np
+    import torch
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    M, F = out.size(-2), out.size(-1)
+    rows = max(1, min(M, (32 << 20) // world // (4 * F)))
+    idx = torch.randperm(M, generator=torch.Generator().manual_seed(1234 + rank))[:rows].sort().values
+    np.save(d / f"spmm_out_rank{rank}.npy", out[idx.to(out.device)].float().cpu().numpy())
+    np.save(d / f"spmm_out_rows_rank{rank}.npy", idx.double().numpy())
+
+
 def run_ours(args, w):
     import torch
     import torch.distributed as dist
@@ -351,6 +369,8 @@ def run_ours(args, w):
     ev1.record()
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out, rank, world)
     if world > 1:
         dist.barrier()
 
@@ -465,7 +485,7 @@ def run_ours(args, w):
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         peaks = json.loads(pk.read_text())
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))   # fallback: H100 SXM data-sheet HBM3 bandwidth (not measured)
 
     secondary = None
     if world == 1 and not args.no_secondary and args.workload == "c2":
@@ -497,8 +517,9 @@ def run_ours(args, w):
             "config": {"workload": w["desc"], "rows_per_gpu": M, "cols": N, "nnz_per_gpu": E, "F": F,
                        "reduce": reduce, "parallelism": f"row-block x{world}; headline = steady state (dense operand "
                        f"already gathered); the including-gather step is in `multi_gpu`" if world > 1 else "single GPU",
-                       "l2": "inputs larger than L2 (dense operand %d MB + indices %d MB vs 126 MB L2); no flush"
-                             % (s * N * F >> 20, (8 * E + s * E) >> 20),
+                       "l2": "dense operand %d MB + indices %d MB vs %d MB L2; no flush"
+                             % (s * N * F >> 20, (8 * E + s * E) >> 20,
+                                torch.cuda.get_device_properties(dev).L2_cache_size >> 20),
                        "accumulate": "fp32",
                        "plan": "segment structure of the matrix planned once (tsb200_spmm_plan, cached per rowptr "
                                "like csr2csc): every timed step is one memset + one kernel"},
@@ -751,6 +772,8 @@ def main():
     ap.add_argument("--workload", default="c2", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the secondary north_star targets (N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's output as .npy files into DIR")
     args = ap.parse_args()
     w = WORKLOADS[args.workload]
     if args.impl == "reference":

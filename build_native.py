@@ -1,4 +1,4 @@
-"""Build libtsb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libtsb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python build_native.py [--force] [--verbose]
 
@@ -27,8 +27,9 @@ LIB = PKG / "libtsb200.so"
 
 SOURCES = ["spmm_fw.cu", "spmm_bw.cu", "convert.cu", "coalesce.cu", "spspmm.cu", "host_api.cu"]
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "-cudart", "shared",
@@ -77,7 +78,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         objs = list(ex.map(lambda s: _compile(s, force, verbose), SOURCES))
     newest = max(o.stat().st_mtime_ns for o in objs)
     if force or not LIB.exists() or LIB.stat().st_mtime_ns < newest:
-        cmd = [_nvcc(), "-shared", "-cudart", "shared", "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [_nvcc(), "-shared", "-cudart", "shared", *GENCODE,
                "-Xlinker", "-rpath", "-Xlinker", "/usr/local/cuda/lib64",
                "-o", str(LIB), *map(str, objs)]
         res = subprocess.run(cmd, capture_output=True, text=True)

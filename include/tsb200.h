@@ -1,5 +1,5 @@
 /*
- * tsb200.h — C-ABI of libtsb200.so: the B200-native (sm_100a) implementation of the
+ * tsb200.h — C-ABI of libtsb200.so: the H100-native (sm_90a) implementation of the
  * torch_sparse sparse-matmul hot path (CSR SpMM fwd/bwd, COO coalesce, SpSpMM, CSR<->COO/CSC
  * format kernels).
  *
@@ -63,7 +63,7 @@ typedef enum { TSB200_SUM = 0, TSB200_MEAN = 1, TSB200_MIN = 2, TSB200_MAX = 3 }
 
 TSB200_API int tsb200_version(void);
 TSB200_API const char* tsb200_strerror(int code);
-/* 0 iff a CUDA device with compute capability 10.x is current. */
+/* 0 iff a CUDA device with compute capability 9.x is current. */
 TSB200_API int tsb200_device_ok(void);
 /* CUDA toolkit version the library was built with, CUDA_VERSION encoding (12090 = 12.9). Replaces
  * torch.ops.torch_sparse.cuda_version() (csrc/version.cpp:27-41), read by the import-time check at

@@ -9,8 +9,8 @@ Recipe: g++ directly on those files against the installed libtorch headers (no s
 flags as the reference's setup.py:67-83 (-O3 -fopenmp -DAT_PARALLEL_OPENMP). OpenMP is NOT passed
 at link time (this image's g++ has no libgomp.spec; libtorch already provides libgomp).
 
-oracle/_ref is git-ignored but travels to the GPU box with the snapshot. TEST / BASELINE
-INFRASTRUCTURE ONLY (see oracle/__init__.py).
+oracle/_ref is git-ignored. BASELINE INFRASTRUCTURE ONLY: bench.py's CPU baseline times these operators when they
+were built, and oracle/gen_golden.py records their outputs under tests/golden/ (see oracle/__init__.py).
 """
 from __future__ import annotations
 
@@ -56,20 +56,12 @@ def _one(item):
     return so
 
 
-REF_TESTS = ["test_matmul.py", "test_spmm.py", "test_spspmm.py", "test_coalesce.py", "test_storage.py",
-             "test_transpose.py", "test_add.py", "test_mul.py", "test_tensor.py", "test_overload.py"]
-
-
-def stage_tests() -> Path:
-    """Stage the reference's own test files for the hot path, byte for byte, next to its compiled operators in
-    oracle/_ref/ref_tests/ (git-ignored: they never enter this repo's history, but travel to the GPU box, where
-    tests/test_reference_suite_gpu.py runs them unmodified against pytorch_sparse_b200)."""
-    import shutil
-    dst = OUT / "ref_tests"
-    dst.mkdir(parents=True, exist_ok=True)
-    for name in REF_TESTS:
-        shutil.copyfile(REF / "test" / name, dst / name)
-    return dst
+def sources_present() -> bool:
+    """True when the reference's sources can be read here (a tree this user may not read counts as absent)."""
+    try:
+        return (REF / "csrc/cpu/spmm_cpu.cpp").is_file()
+    except OSError:
+        return False
 
 
 def build() -> Path:
@@ -78,7 +70,6 @@ def build() -> Path:
     OUT.mkdir(parents=True, exist_ok=True)
     with ThreadPoolExecutor(max_workers=3) as ex:
         list(ex.map(_one, LIBS.items()))
-    stage_tests()
     return OUT
 
 

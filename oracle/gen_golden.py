@@ -390,9 +390,42 @@ def gen_grads(ts, meta):
     print("grads.pt", (GOLD / "grads.pt").stat().st_size)
 
 
+def gen_reference_ops(meta):
+    """The reference's compiled CPU operators (ind2ptr / ptr2ind, spmm_sum / mean / min / max) on a batched dense
+    operand ([2, N, K]) in every dtype the oracle is pinned to bit for bit (tests/test_oracle_pinning.py)."""
+    from oracle import build_ref
+    build_ref.build()
+    build_ref.load()
+    ops = torch.ops.torch_sparse
+    g = torch.Generator().manual_seed(0)
+    M, N, K = 40, 30, 4
+    deg = torch.randint(0, 8, (M,), generator=g)
+    row = torch.repeat_interleave(torch.arange(M), deg)
+    col = torch.randint(N, (row.numel(),), generator=g)
+    rowptr = ops.ind2ptr(row, M)
+    out = {"meta": meta, "row": row, "col": col, "M": M, "rowptr": rowptr,
+           "ptr2ind": ops.ptr2ind(rowptr, row.numel()), "cases": {}}
+    for dt in (torch.float32, torch.float64, torch.bfloat16, torch.float16, torch.int64):
+        if dt.is_floating_point:
+            v = torch.randn(col.numel(), generator=g).to(dt)
+            x = torch.randn(2, N, K, generator=g).to(dt)
+        else:
+            v = torch.randint(-5, 6, (col.numel(),), generator=g)
+            x = torch.randint(-5, 6, (2, N, K), generator=g)
+        c = {"value": v, "mat": x,
+             "sum": ops.spmm_sum(None, rowptr, col, v, None, None, x),
+             "mean": ops.spmm_mean(None, rowptr, col, v, None, None, None, x)}
+        c["min"], c["argmin"] = ops.spmm_min(rowptr, col, v, x)
+        c["max"], c["argmax"] = ops.spmm_max(rowptr, col, v, x)
+        out["cases"][str(dt).split(".")[-1]] = c
+    torch.save(out, GOLD / "reference_ops.pt")
+
+
 if __name__ == "__main__":
     _meta = {"reference": "rusty1s/pytorch_sparse 0.6.18 @ 91feaa5e", "torch": torch.__version__}
-    if len(sys.argv) > 1 and sys.argv[1] == "spspmm2":
+    if len(sys.argv) > 1 and sys.argv[1] == "reference_ops":
+        gen_reference_ops(_meta)
+    elif len(sys.argv) > 1 and sys.argv[1] == "spspmm2":
         gen_spspmm2(import_reference(), _meta)
     elif len(sys.argv) > 1 and sys.argv[1] == "next_rows2":
         gen_next_rows2(import_reference(), {"reference": "rusty1s/pytorch_sparse 0.6.18 @ 91feaa5e", "torch": torch.__version__})

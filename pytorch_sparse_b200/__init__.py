@@ -1,4 +1,4 @@
-"""pytorch_sparse_b200 — a from-scratch, Blackwell-native (sm_100a) implementation of the
+"""pytorch_sparse_b200 — a from-scratch, Hopper-native (sm_90a) implementation of the
 torch_sparse sparse-matmul hot path (CSR SpMM fwd/bwd, COO coalesce, SpSpMM) behind the
 reference's own `SparseTensor` / `(index, value)` API.
 

@@ -77,7 +77,7 @@ def _load() -> ctypes.CDLL:
     if not LIB_PATH.exists():
         raise ImportError(
             f"pytorch_sparse_b200: {LIB_PATH} is missing. Build it with "
-            f"`python build_native.py` (needs nvcc, sm_100a). There is no fallback path.")
+            f"`python build_native.py` (needs nvcc, sm_90a). There is no fallback path.")
     try:
         lib = ctypes.CDLL(str(LIB_PATH), mode=ctypes.RTLD_GLOBAL)
     except OSError as e:  # pragma: no cover

@@ -1,4 +1,4 @@
-// coalesce.cu — COO coalesce for sm_100a.
+// coalesce.cu — COO coalesce for sm_90a.
 //
 // Replaces torch_sparse.coalesce -> SparseStorage.__init__ (sort) + SparseStorage.coalesce()
 // (torch_sparse/coalesce.py:5-25, torch_sparse/storage.py:149-162, 436-466; value reduction =

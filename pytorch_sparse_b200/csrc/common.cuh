@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the libtsb200 kernels (sm_100a only).
+// common.cuh — shared helpers for the libtsb200 kernels (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -26,7 +26,7 @@
 
 namespace tsb {
 
-constexpr int kDefaultSMs = 148;  // B200: 2 dies x 74 SMs (used only if the attribute query fails)
+constexpr int kDefaultSMs = 132;  // H100 SXM (used only if the attribute query fails)
 constexpr int kMaxDevices = 64;
 
 // SM count of the CURRENT device, queried once per device and cached (thread-safe: idempotent atomic stores).

@@ -1,4 +1,4 @@
-// convert.cu — CSR/COO/CSC format kernels for sm_100a.
+// convert.cu — CSR/COO/CSC format kernels for sm_90a.
 //
 //  * tsb200_ind2ptr / tsb200_ptr2ind replace torch.ops.torch_sparse.{ind2ptr,ptr2ind}
 //    (csrc/convert.cpp:22-48, csrc/cpu/convert_cpu.cpp:7-57, csrc/cuda/convert_cuda.cu:9-67).

@@ -3,10 +3,10 @@
 // tensors, cf. spmm_cpu(rowptr, col, value, mat, reduce), csrc/cpu/spmm_cpu.cpp:8-11).
 //
 // tsb200_spmm_fw_host pipelines PCIe against the kernel: `mat` goes up first, split over TWO upload
-// streams (one DMA stream tops out at ~40 GB/s H2D on these hosts, two reach ~51 GB/s), then the CSR
-// arrays in row chunks alternating between the two; each chunk's SpMM starts on a compute stream as soon
-// as its indices have landed and its output rows are copied back on a fourth stream while later chunks
-// are still uploading (the link sustains ~87 GB/s bidirectional).
+// streams (one DMA stream does not saturate the host link), then the CSR arrays in row chunks alternating
+// between the two; each chunk's SpMM starts on a compute stream as soon as its indices have landed and its
+// output rows are copied back on a fourth stream while later chunks are still uploading (the link is
+// full duplex).
 #include <cstdlib>
 #include <mutex>
 
@@ -71,7 +71,7 @@ extern "C" const char* tsb200_strerror(int code) {
     case TSB200_ERR_INVALID_ARG: return "tsb200: invalid argument";
     case TSB200_ERR_UNSUPPORTED: return "tsb200: unsupported dtype/reduce/extent combination";
     case TSB200_ERR_WORKSPACE: return "tsb200: workspace missing or too small";
-    case TSB200_ERR_NO_DEVICE: return "tsb200: no sm_100 CUDA device";
+    case TSB200_ERR_NO_DEVICE: return "tsb200: no sm_90 CUDA device";
   }
   if (code > 0) return cudaGetErrorString((cudaError_t)code);
   return "tsb200: unknown error";
@@ -83,7 +83,7 @@ extern "C" int tsb200_device_ok(void) {
   int major = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
     return TSB200_ERR_NO_DEVICE;
-  return major == 10 ? 0 : TSB200_ERR_NO_DEVICE;
+  return major == 9 ? 0 : TSB200_ERR_NO_DEVICE;
 }
 
 static int spmm_fw_host_locked(HostCtx& c, const int64_t* rowptr_host, const int64_t* col_host,

@@ -1,4 +1,4 @@
-// spmm_bw.cu — SpMM backward kernels for sm_100a.
+// spmm_bw.cu — SpMM backward kernels for sm_90a.
 //
 //  * tsb200_spmm_value_bw: SDDMM  out[e] = sum_b <mat[b,col[e],:], grad[b,row[e],:]>
 //    replaces spmm_value_bw_cpu / spmm_value_bw_kernel
@@ -23,31 +23,25 @@ template <> struct Vec16<float, 4> {
            __uint_as_float(a.z) * __uint_as_float(b.z) + __uint_as_float(a.w) * __uint_as_float(b.w);
   }
 };
-// bf16 / f16: sm_100 mixed-precision FMA (fma.rn.f32.{bf16,f16} -> SASS FHFMA with .H0/.H1 selectors):
-// both multiplicands straight from the packed pairs, fp32 accumulate, no unpack.
-template <> struct Vec16<__nv_bfloat16, 8> {
-  static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) {
-    const uint32_t x[4] = {a.x, a.y, a.z, a.w}, y[4] = {b.x, b.y, b.z, b.w};
-    float s0 = 0.f, s1 = 0.f;
+// bf16 / f16: both operands widened to fp32 (exact, Vec<T>::unpack), products of two 16-bit values are exact in
+// fp32, so FFMA rounds once per term; even and odd lanes of the pairs accumulate separately, fp32 throughout.
+template <typename T> __device__ __forceinline__ float dot16(const uint4& a, const uint4& b) {
+  float x[8], y[8];
+  Vec<T>::unpack(a, x);
+  Vec<T>::unpack(b, y);
+  float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-    for (int i = 0; i < 4; i++)
-      asm("{\n\t.reg .b16 al, ah, bl, bh;\n\tmov.b32 {al, ah}, %2;\n\tmov.b32 {bl, bh}, %3;\n\t"
-          "fma.rn.f32.bf16 %0, al, bl, %0;\n\tfma.rn.f32.bf16 %1, ah, bh, %1;\n\t}"
-          : "+f"(s0), "+f"(s1) : "r"(x[i]), "r"(y[i]));
-    return s0 + s1;
+  for (int i = 0; i < 4; i++) {
+    s0 = fmaf(x[2 * i], y[2 * i], s0);
+    s1 = fmaf(x[2 * i + 1], y[2 * i + 1], s1);
   }
+  return s0 + s1;
+}
+template <> struct Vec16<__nv_bfloat16, 8> {
+  static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) { return dot16<__nv_bfloat16>(a, b); }
 };
 template <> struct Vec16<__half, 8> {
-  static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) {
-    const uint32_t x[4] = {a.x, a.y, a.z, a.w}, y[4] = {b.x, b.y, b.z, b.w};
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-      asm("{\n\t.reg .b16 al, ah, bl, bh;\n\tmov.b32 {al, ah}, %2;\n\tmov.b32 {bl, bh}, %3;\n\t"
-          "fma.rn.f32.f16 %0, al, bl, %0;\n\tfma.rn.f32.f16 %1, ah, bh, %1;\n\t}"
-          : "+f"(s0), "+f"(s1) : "r"(x[i]), "r"(y[i]));
-    return s0 + s1;
-  }
+  static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) { return dot16<__half>(a, b); }
 };
 
 // Reduce U per-lane partial sums over the W*2 lanes of a lane group with a halving butterfly:
@@ -187,11 +181,11 @@ template <typename T, int LPR, int CH, int U> struct SddmmEngine {
       const int jrel = jend - j0 - g;
       uint4 d[U][CH];
       float part[U];
-      // Branch-free chunk (the kernel is issue-bound, profiles/r01_ncu_late_captures.md: ~35 of its ~250 instructions
-      // per chunk were branches around the inline-asm gathers): the gathers are predicated inside the asm into zeroed
+      // Branch-free chunk (the kernel is issue-bound, and branches around the inline-asm gathers cost issue slots):
+      // the gathers are predicated inside the asm into zeroed
       // registers and the dot products run unconditionally (an inactive slot contributes 0). The ring slot is read
       // unconditionally — slots past the row's end hold stale but in-bounds column words, and the predicate keeps
-      // them from being dereferenced. Measured on B200 at C2: 0.735 -> 0.571 ms (profiles/r02_results.md).
+      // them from being dereferenced.
 #pragma unroll
       for (int u = 0; u < U; u++) {
         const bool act = (u < nst) && (u * G < jrel);
@@ -549,15 +543,17 @@ extern "C" int tsb200_spmm_minmax_bw(const int64_t* col, const void* value, cons
   return dispatch_float_dtype(dtype, [&](auto tag) -> int {
     using T = decltype(tag);
     using A = typename std::conditional<std::is_same<T, double>::value, double, float>::type;
-    // feature slice (measured at C3, scripts/sweep_minmax_bw.py -> profiles/r01_minmax_bw_sweep.txt): whole rows while
-    // mat + grad_mat fit L2; otherwise 256-byte slices of a row when both gradients are wanted (2.47 -> 1.95 ms),
-    // 128-byte slices (one L2 line; narrower slices waste line capacity and are slower) for a single gradient
-    // (grad_mat only: 1.62 -> 1.16 ms)
+    // feature slice (scripts/sweep_minmax_bw.py): whole rows while mat + grad_mat fit in half of L2; otherwise
+    // 256-byte slices of a row when both gradients are wanted, 128-byte slices (one L2 line; narrower slices waste
+    // line capacity) for a single gradient
     int full = 0;
     while (((int64_t)1 << full) < K) full++;
     int lsl = full;
+    int dev = 0, l2 = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) != cudaSuccess)
+      l2 = 0;
     const double resident = (double)B * (double)N * (double)K * (double)(sizeof(T) + sizeof(A));
-    if (resident > 64.0 * 1024 * 1024) {
+    if (resident > 0.5 * (double)l2) {
       const int slice_bytes = (grad_value && grad_mat) ? 256 : 128;
       lsl = 0;
       while ((size_t)(2u << lsl) * sizeof(T) <= (size_t)slice_bytes) lsl++;

@@ -139,8 +139,9 @@ template <typename T> struct IndexRing {
 
 // ---- accumulator helpers -----------------------------------------------------------------------
 // Vec<T>: how one 16-byte gather of T is folded into fp32 accumulators.
-//   * bf16 / f16 use the sm_100 mixed-precision FMA (PTX fma.rn.f32.{bf16,f16} -> SASS FHFMA with
-//     .H0/.H1 operand selectors): fp32 accumulate straight from the packed 16-bit pairs, no unpack.
+//   * bf16 / f16: both halves of a packed pair are widened to fp32 (exact: a bf16 widens with a shift or a mask,
+//     an f16 with one conversion) and folded with FFMA. The product of two 16-bit values is exact in fp32, so this
+//     rounds once per term, exactly like a fused mixed-precision FMA would.
 //   * the nnz value travels as the raw storage bits (`vraw`), 1.0 when has_value=false.
 template <typename T> struct Vec;
 template <> struct Vec<float> {
@@ -169,14 +170,12 @@ template <> struct Vec<__nv_bfloat16> {
   using vraw = unsigned short;
   static __device__ __forceinline__ vraw one() { return 0x3F80; }
   static __device__ __forceinline__ float vfloat(vraw v) { return __uint_as_float((uint32_t)v << 16); }
-  static __device__ __forceinline__ void fma2(float& a0, float& a1, vraw v, uint32_t w) {
-    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %3;\n\t"
-        "fma.rn.f32.bf16 %0, %2, lo, %0;\n\tfma.rn.f32.bf16 %1, %2, hi, %1;\n\t}"
-        : "+f"(a0), "+f"(a1) : "h"(v), "r"(w));
-  }
   static __device__ __forceinline__ void fma(float* acc, vraw v, const uint4& d) {
-    fma2(acc[0], acc[1], v, d.x); fma2(acc[2], acc[3], v, d.y);
-    fma2(acc[4], acc[5], v, d.z); fma2(acc[6], acc[7], v, d.w);
+    const float vf = vfloat(v);
+    float f[VEC];
+    unpack(d, f);
+#pragma unroll
+    for (int i = 0; i < VEC; i++) acc[i] = fmaf(vf, f[i], acc[i]);
   }
   static __device__ __forceinline__ void unpack(const uint4& d, float* f) {
     const uint32_t w[4] = {d.x, d.y, d.z, d.w};
@@ -202,14 +201,12 @@ template <> struct Vec<__half> {
   using vraw = unsigned short;
   static __device__ __forceinline__ vraw one() { return 0x3C00; }
   static __device__ __forceinline__ float vfloat(vraw v) { return __half2float(__ushort_as_half(v)); }
-  static __device__ __forceinline__ void fma2(float& a0, float& a1, vraw v, uint32_t w) {
-    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %3;\n\t"
-        "fma.rn.f32.f16 %0, %2, lo, %0;\n\tfma.rn.f32.f16 %1, %2, hi, %1;\n\t}"
-        : "+f"(a0), "+f"(a1) : "h"(v), "r"(w));
-  }
   static __device__ __forceinline__ void fma(float* acc, vraw v, const uint4& d) {
-    fma2(acc[0], acc[1], v, d.x); fma2(acc[2], acc[3], v, d.y);
-    fma2(acc[4], acc[5], v, d.z); fma2(acc[6], acc[7], v, d.w);
+    const float vf = vfloat(v);
+    float f[VEC];
+    unpack(d, f);
+#pragma unroll
+    for (int i = 0; i < VEC; i++) acc[i] = fmaf(vf, f[i], acc[i]);
   }
   static __device__ __forceinline__ void unpack(const uint4& d, float* f) {
     const uint32_t w[4] = {d.x, d.y, d.z, d.w};
@@ -256,9 +253,8 @@ static inline WsLayout ws_layout(int64_t B, int64_t K, int64_t E, bool arg, bool
   return L;
 }
 
-// Policy choice for the dense operand (host side). An operand that fits into L2 twice over keeps the blanket
-// evict_last; a larger one gets a pinned slice of kPinBytes (tuned on B200, profiles/r02_l2_policy_sweep.txt;
-// TSB200_PIN_MB overrides, 0 = blanket evict_last).
+// Policy choice for the dense operand (host side). By default every gather carries the blanket evict_last;
+// TSB200_PIN_MB=<n> instead pins the first n MB of a larger operand and streams the rest (0 = blanket evict_last).
 constexpr size_t kPinBytesDefault = 0;
 static inline void choose_pin(SpmmParams& p, size_t mat_bytes) {
   p.pin_bytes = 0;

@@ -1,11 +1,11 @@
-// spmm_fw.cu — CSR SpMM forward for sm_100a.
+// spmm_fw.cu — CSR SpMM forward for sm_90a.
 //
 // Replaces spmm_fw -> spmm_cpu / spmm_cuda of the reference
 // (csrc/spmm.cpp:22-35, csrc/cpu/spmm_cpu.cpp:8-101, csrc/cuda/spmm_cuda.cu:13-155).
 //
 // Design (row-split CSR, HBM/L2-gather bound; see DESIGN.md §SpMM):
 //   * work item = 32 consecutive rows, pulled by a WARP from a global atomic counter
-//     (persistent grid: 148 SMs x resident CTAs);
+//     (persistent grid: every SM x resident CTAs);
 //   * the item's rowptr slice lives in lane registers (one coalesced 264 B read);
 //   * col/value of the item's contiguous nnz range stream through a per-warp shared-memory
 //     ring filled by cp.async (LDGSTS) 32-entry windows, issued 2 windows ahead of use, so the
@@ -576,8 +576,7 @@ spmm_vec_kernel(const SpmmParams p) {
 
 // ---- narrow dense rows (K*sizeof(T) <= 128 B): group-per-row SUM kernel ----------------------------
 // With LPR <= 8 a row-at-a-time warp spends most of its instructions on per-row bookkeeping and on the
-// cross-group reduction (profiles/r01_ncu_spmm_f32.md: 308 warp-instructions per 16-nnz row, issue
-// slots 87 % busy). Here the G = 32/LPR lane groups of a warp each walk their OWN row: no cross-group
+// cross-group reduction (the kernel becomes issue-bound). Here the G = 32/LPR lane groups of a warp each walk their OWN row: no cross-group
 // reduction, per-row overhead amortised over G rows, U independent (index -> gather) chains in flight
 // per lane. Indices are read straight from global memory (lanes of a group broadcast one address,
 // consecutive nnz hit L1). Long rows / budget overflow still go to the segment queue.
@@ -967,8 +966,8 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
 }
 
 // (LPR, CH) follow from the width of a dense row; (U, MINB) = gathers in flight per lane and CTAs
-// per SM, tuned on B200 (profiles/r01_variant_sweep.txt): the kernel is HBM-latency bound, so
-// resident warps x gathers-in-flight wins; 40 warps/SM x 4 x 16 B per lane saturates HBM.
+// per SM: the kernel is HBM-latency bound, so resident warps x gathers-in-flight wins (40 warps/SM x 4 x 16 B
+// per lane; the register budget of MINB = 5 is the same 64K registers per SM on sm_90).
 template <typename T, int RED, bool ACC = false, bool PLAN = false> static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(T);
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row

@@ -1,4 +1,4 @@
-// spspmm.cu — CSR x CSR -> CSR/COO sparse-sparse matmul for sm_100a.
+// spspmm.cu — CSR x CSR -> CSR/COO sparse-sparse matmul for sm_90a.
 //
 // Replaces spspmm_sum -> torch.sparse.mm (torch_sparse/matmul.py:94-111; CPU: ATen sparse_matmul,
 // CUDA: cuSPARSE SpGEMM), keeping its observable contract: output sorted by (row, col), unique,
@@ -16,8 +16,8 @@
 //   * FLAT rows (single window, <= 128 A entries, <= 2048 products; every row of BASELINE's C4): the row's
 //     products are numbered 0..P-1 through a prefix sum of the B-row lengths and dealt to the threads
 //     (chunks of 32 round-robin over the warps, <= 8 products per thread), which keep them in REGISTERS across the passes, so B is read once per phase and every lane
-//     is busy whatever the B-row lengths are. Bits are set with plain LDS/STS (shared-memory atomics cost
-//     2 cycles PER LANE on sm_100: 64 cycles per scattered warp-wide ATOMS.OR, 1.9 ms per pass at C4);
+//     is busy whatever the B-row lengths are. Bits are set with plain LDS/STS (a scattered warp-wide
+//     shared-memory ATOMS.OR is serialised lane by lane);
 //     two writers racing on one WORD can lose a bit, so after a barrier every product checks its own bit
 //     and repairs a loss with an atomicOr (atomics only add bits, so the repair pass is race-free and only
 //     the rare losers pay). The output row is staged in shared memory -- one word per slot carries the

@@ -560,7 +560,7 @@ def spspmm(rowptr_a: Tensor, col_a: Tensor, val_a: Optional[Tensor], rowptr_b: T
     esize = 0 if not want_value else (8 if dtype == torch.float64 else 4)
     # two_phase (symbolic + numeric kernels) is the default. "fused" selects the single-pass kernel (rows placed by
     # a decoupled look-back, outputs sized by the product bound): bit-identical structure, one kernel instead of two,
-    # but measured slower on B200 at C4 (6.2 vs 6.0 ms, profiles/r02_spspmm_single_pass.md) — kept as an option.
+    # kept as an option.
     mode = os.environ.get("TSB200_SPSPMM", "two_phase")
     with _on_device(dev):
         nws = lib.tsb200_spspmm_workspace_bytes(M, Kd, N, nnz_a, nnz_b)

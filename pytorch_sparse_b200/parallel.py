@@ -155,13 +155,13 @@ class PipelinedRowShardedSpMM:
     the slice-major layout on both sides (`forward_sliced`: [C, block, F/C] in, [C, M, F/C] out), which is what a
     chain of layers wants: the output of one step is already laid out for the gather of the next.
     split="column": A's columns are split instead (`split_column_chunks`) and the chunks share an fp32 partial
-    (tsb200_spmm_fw_acc). Measured slower — every chunk re-walks the row structure and read-modify-writes the
-    partial (profiles/r02_results.md) — kept for operands that cannot be sliced by features.
+    (tsb200_spmm_fw_acc). Every chunk re-walks the row structure and read-modify-writes the partial, so it is kept
+    for operands that cannot be sliced by features.
 
     transport="peer" (default on CUDA/NCCL groups): every rank keeps its slices in a symmetric-memory buffer and PULLS
     the peers' slices with cudaMemcpyAsync over NVLink — copy engines only. The SpMM kernel is a persistent grid that
     fills every SM, so a transfer that needs SMs (NCCL's all-gather kernel) cannot run beside it and the "overlap"
-    serialises; DMA pulls do overlap (profiles/r02_results.md). transport="nccl": chunked all_gather_into_tensor."""
+    serialises; DMA pulls do overlap. transport="nccl": chunked all_gather_into_tensor."""
 
     def __init__(self, a_local: SparseTensor, block: int, chunks: int = 4, group=None, split: str = "feature",
                  transport: str = "auto"):
@@ -170,8 +170,7 @@ class PipelinedRowShardedSpMM:
             transport = "peer" if (a_local.is_cuda() and split == "feature" and _world(group) > 1
                                    and dist.get_backend(group) == "nccl") else "nccl"
         self.transport = transport
-        # concurrent DMA streams of the pulls: ONE is fastest at N = 8 (3.39 ms vs 5.78 / 4.91 ms with 2 / 7 streams:
-        # concurrent peer copies contend), and as fast as any at N = 2 (profiles/r02_results.md)
+        # concurrent DMA streams of the pulls (default one: concurrent peer copies contend)
         self.peer_streams = int(os.environ.get("TSB200_PEER_STREAMS", "1"))
         self.group = group
         self.world = _world(group)

@@ -132,16 +132,6 @@ __device__ __forceinline__ uint64_t make_policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-// Range policy over the dense operand: the first `primary_bytes` of [base, base + total_bytes) are kept with
-// evict_last, the rest is streamed with evict_first. When the operand is larger than L2 a blanket evict_last protects
-// nothing from itself (every line has the same priority); pinning a fixed slice that FITS turns that slice's
-// gathers into guaranteed hits and lets the remainder stream past it.
-__device__ __forceinline__ uint64_t make_policy_range(const void* base, uint32_t primary_bytes, uint32_t total_bytes) {
-  uint64_t pol;
-  asm volatile("createpolicy.range.global.L2::evict_last.L2::evict_first.b64 %0, [%1], %2, %3;"
-               : "=l"(pol) : "l"(base), "r"(primary_bytes), "r"(total_bytes));
-  return pol;
-}
 __device__ __forceinline__ uint64_t make_policy_evict_first() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));

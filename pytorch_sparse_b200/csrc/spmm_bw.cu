@@ -496,7 +496,7 @@ extern "C" int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
       SpmmParams p;
       p.rowptr = rowptr; p.col = col; p.value = nullptr; p.mat = mat; p.out = nullptr; p.arg_out = nullptr;
       p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = mean ? 1 : 0; p.item_shift = 5;
-      p.partial = nullptr; p.acc_mode = 0; p.pin_bytes = 0; p.mat_bytes = 0;
+      p.partial = nullptr; p.acc_mode = 0;
       p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
       p.counters = (unsigned int*)(ws + L.counters);
       p.segs = (Segment*)(ws + L.segs);

@@ -2,8 +2,6 @@
 // work-queue records, kernel parameters, the per-warp cp.async index ring and the 16-byte vector math.
 #pragma once
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace tsb {
@@ -44,9 +42,6 @@ struct SpmmParams {
   // A that share an fp32 partial [B, M, K]:  1 = write the partial, 2 = add to it, 3 = add to it and write `out`
   float* partial;
   int acc_mode;
-  // L2 residency of the dense operand: 0 = evict_last on every gather; otherwise the first pin_bytes of `mat`
-  // (total mat_bytes < 4 GB) are evict_last and the rest evict_first (make_policy_range)
-  uint32_t pin_bytes, mat_bytes;
   // planned mode (tsb200_spmm_plan, B == 1): which rows go through the segment list is known up front — bit r of
   // plan_mask[r / 32] — the list itself (segs / longs above) lives in the plan, its sizes are host-known, and the
   // main kernel drains it itself once the row items are gone (no segment / combine launches)
@@ -251,22 +246,6 @@ static inline WsLayout ws_layout(int64_t B, int64_t K, int64_t E, bool arg, bool
   L.part_arg = off; off += (partials && arg) ? align_up((size_t)L.slot_cap * (size_t)K * sizeof(int64_t), 256) : 0;
   L.total = off;
   return L;
-}
-
-// Policy choice for the dense operand (host side). By default every gather carries the blanket evict_last;
-// TSB200_PIN_MB=<n> instead pins the first n MB of a larger operand and streams the rest (0 = blanket evict_last).
-constexpr size_t kPinBytesDefault = 0;
-static inline void choose_pin(SpmmParams& p, size_t mat_bytes) {
-  p.pin_bytes = 0;
-  p.mat_bytes = 0;
-  size_t pin = kPinBytesDefault;
-  if (const char* ev = getenv("TSB200_PIN_MB")) pin = (size_t)atol(ev) << 20;
-  if (pin == 0 || mat_bytes >= ((size_t)1 << 32) || mat_bytes <= pin) return;
-  p.pin_bytes = (uint32_t)pin;
-  p.mat_bytes = (uint32_t)mat_bytes;
-}
-__device__ __forceinline__ uint64_t mat_policy(const SpmmParams& p) {
-  return p.pin_bytes ? make_policy_range(p.mat, p.pin_bytes, p.mat_bytes) : make_policy_evict_last();
 }
 
 static inline int grid_for(const void* kernel, int threads) {

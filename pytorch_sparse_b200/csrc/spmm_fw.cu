@@ -422,7 +422,7 @@ spmm_vec_kernel(const SpmmParams p) {
   ring.col = p.col;
   ring.val = (const T*)p.value;
   ring.limit = p.E;
-  const uint64_t pol = mat_policy(p);
+  const uint64_t pol = make_policy_evict_last();
 
   bool col_ok[CH];
 #pragma unroll
@@ -602,7 +602,7 @@ spmm_gpr_kernel(const SpmmParams p) {
   const bool col_ok = p.k0 + li * VEC < p.K;
   const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
   const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(T);
-  const uint64_t pol = mat_policy(p);
+  const uint64_t pol = make_policy_evict_last();
   const T* __restrict__ val = (const T*)p.value;
   const bool has_val = val != nullptr;
 
@@ -763,7 +763,7 @@ spmm_seg_kernel(const SpmmParams p) {
   ring.col = p.col;
   ring.val = (const T*)p.value;
   ring.limit = p.E;
-  const uint64_t pol = mat_policy(p);
+  const uint64_t pol = make_policy_evict_last();
 
   bool col_ok[CH];
 #pragma unroll
@@ -1139,7 +1139,6 @@ extern "C" int tsb200_spmm_fw(const int64_t* rowptr, const int64_t* col, const v
     p.B = B; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
     p.partial = nullptr; p.acc_mode = 0;
     p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-    choose_pin(p, (size_t)B * N * K * dtype_size(dtype));
     p.counters = (unsigned int*)(ws + L.counters);
     p.segs = (Segment*)(ws + L.segs);
     p.longs = (LongRow*)(ws + L.longs);
@@ -1189,7 +1188,6 @@ extern "C" int tsb200_spmm_fw_acc(const int64_t* rowptr, const int64_t* col, con
   p.B = B; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
   p.partial = partial; p.acc_mode = acc_mode;
   p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-  choose_pin(p, (size_t)B * N * K * dtype_size(dtype));
   p.counters = (unsigned int*)(ws + L.counters);
   p.segs = (Segment*)(ws + L.segs);
   p.longs = (LongRow*)(ws + L.longs);
@@ -1268,7 +1266,6 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
   p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
   p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
   p.partial = nullptr; p.acc_mode = 0;
-  choose_pin(p, (size_t)N * K * dtype_size(dtype));
   p.counters = (unsigned int*)(ws + W.counters);
   p.long_done = (uint32_t*)(ws + W.long_done);   // directly behind the counters: one memset clears both
   p.segs = (Segment*)(pl + PL.segs);

@@ -486,7 +486,7 @@ extern "C" int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
   const bool vec = (dtype == TSB200_F32 || dtype == TSB200_F16 || dtype == TSB200_BF16) && K > 0 &&
                    (K * es) % 16 == 0 && !((uintptr_t)mat & 15) && !((uintptr_t)grad & 15) &&
                    M < ((int64_t)1 << 32) && N < ((int64_t)1 << 32) && K * (int64_t)es < ((int64_t)1 << 31);
-  // row-wise path: single batch, >= 4 and <= 64 vectors per dense row, a workspace for the segment queue
+  // row-wise path: single batch, >= 3 and <= 64 vectors per dense row, a workspace for the segment queue
   const int64_t vecs = vec ? (K * (int64_t)es) / 16 : 0;
   if (vec && B == 1 && vecs >= 3 && vecs <= 64 && E < ((int64_t)1 << 31) - 64 && !((uintptr_t)col & 7) && workspace &&
       !((uintptr_t)workspace & 255)) {

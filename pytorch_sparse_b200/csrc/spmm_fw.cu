@@ -203,19 +203,24 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
 // ---- packed 16-bit min/max engine --------------------------------------------------------------
 // For bf16 / f16 the reference compares products ROUNDED to the storage type, so the whole min/max
 // recurrence can stay in packed 16-bit pairs: HMUL2 (round-to-nearest product of two pairs), HSETP2
-// (two strict compares -> two predicates, false on NaN like the reference's `>`), HMNMX2 (new extreme) —
-// ~20 instructions per gathered 16-byte vector instead of ~57 for unpack / fp32 multiply / re-round /
-// compare / select. Values are bit-identical to the float path; ties still keep the smallest nnz index.
+// (two strict compares -> two predicates, false on NaN like the reference's `>`), and a per-half select of the
+// new extreme — instead of unpack / fp32 multiply / re-round / compare / select. The extreme is selected by the
+// strict compare, not formed with max.x2 / min.x2: those order -0 below +0, so a later -0 would replace a +0
+// minimum (or +0 a -0 maximum) without moving arg_out. Values are bit-identical to the float path; ties still keep
+// the smallest nnz index.
 template <typename T> struct Pk;
 template <> struct Pk<__nv_bfloat16> {
   static __device__ __forceinline__ uint32_t mul(uint32_t a, uint32_t b) {
     uint32_t r; asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(b)); return r;
   }
-  template <bool MAX> static __device__ __forceinline__ void step(uint32_t& acc, int& a0, int& a1, uint32_t p, int j) {
-    if (MAX) asm("{\n\t.reg .pred q0, q1;\n\tsetp.gt.bf16x2 q0|q1, %3, %2;\n\t@q0 mov.b32 %0, %4;\n\t@q1 mov.b32 %1, %4;\n\t"
-                 "max.bf16x2 %2, %2, %3;\n\t}" : "+r"(a0), "+r"(a1), "+r"(acc) : "r"(p), "r"(j));
-    else asm("{\n\t.reg .pred q0, q1;\n\tsetp.lt.bf16x2 q0|q1, %3, %2;\n\t@q0 mov.b32 %0, %4;\n\t@q1 mov.b32 %1, %4;\n\t"
-             "min.bf16x2 %2, %2, %3;\n\t}" : "+r"(a0), "+r"(a1), "+r"(acc) : "r"(p), "r"(j));
+  // per-half strict compare of product p against the running extreme a (false on NaN): 0xffff in each half that wins
+  template <bool MAX> static __device__ __forceinline__ uint32_t better(uint32_t p, uint32_t a) {
+    uint32_t m;
+    if (MAX) asm("{\n\t.reg .pred q0, q1;\n\tsetp.gt.bf16x2 q0|q1, %1, %2;\n\tselp.b32 %0, 0x0000ffff, 0, q0;\n\t"
+                 "@q1 or.b32 %0, %0, 0xffff0000;\n\t}" : "=r"(m) : "r"(p), "r"(a));
+    else asm("{\n\t.reg .pred q0, q1;\n\tsetp.lt.bf16x2 q0|q1, %1, %2;\n\tselp.b32 %0, 0x0000ffff, 0, q0;\n\t"
+             "@q1 or.b32 %0, %0, 0xffff0000;\n\t}" : "=r"(m) : "r"(p), "r"(a));
+    return m;
   }
   // per-half masks: better (strict) and equal
   template <bool MAX> static __device__ __forceinline__ void cmp(uint32_t o, uint32_t m, bool& b0, bool& b1, bool& e0, bool& e1) {
@@ -238,11 +243,13 @@ template <> struct Pk<__half> {
   static __device__ __forceinline__ uint32_t mul(uint32_t a, uint32_t b) {
     uint32_t r; asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(b)); return r;
   }
-  template <bool MAX> static __device__ __forceinline__ void step(uint32_t& acc, int& a0, int& a1, uint32_t p, int j) {
-    if (MAX) asm("{\n\t.reg .pred q0, q1;\n\tsetp.gt.f16x2 q0|q1, %3, %2;\n\t@q0 mov.b32 %0, %4;\n\t@q1 mov.b32 %1, %4;\n\t"
-                 "max.f16x2 %2, %2, %3;\n\t}" : "+r"(a0), "+r"(a1), "+r"(acc) : "r"(p), "r"(j));
-    else asm("{\n\t.reg .pred q0, q1;\n\tsetp.lt.f16x2 q0|q1, %3, %2;\n\t@q0 mov.b32 %0, %4;\n\t@q1 mov.b32 %1, %4;\n\t"
-             "min.f16x2 %2, %2, %3;\n\t}" : "+r"(a0), "+r"(a1), "+r"(acc) : "r"(p), "r"(j));
+  template <bool MAX> static __device__ __forceinline__ uint32_t better(uint32_t p, uint32_t a) {
+    uint32_t m;
+    if (MAX) asm("{\n\t.reg .pred q0, q1;\n\tsetp.gt.f16x2 q0|q1, %1, %2;\n\tselp.b32 %0, 0x0000ffff, 0, q0;\n\t"
+                 "@q1 or.b32 %0, %0, 0xffff0000;\n\t}" : "=r"(m) : "r"(p), "r"(a));
+    else asm("{\n\t.reg .pred q0, q1;\n\tsetp.lt.f16x2 q0|q1, %1, %2;\n\tselp.b32 %0, 0x0000ffff, 0, q0;\n\t"
+             "@q1 or.b32 %0, %0, 0xffff0000;\n\t}" : "=r"(m) : "r"(p), "r"(a));
+    return m;
   }
   template <bool MAX> static __device__ __forceinline__ void cmp(uint32_t o, uint32_t m, bool& b0, bool& b1, bool& e0, bool& e1) {
     uint32_t x0, x1, y0, y1;
@@ -285,8 +292,13 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
     const uint32_t v2 = P::splat(v);  // 1.0 when has_value=false => exact products
     const uint32_t w[4] = {d.x, d.y, d.z, d.w};
 #pragma unroll
-    for (int k = 0; k < 4; k++)
-      P::template step<MAX>(pacc[ch * 4 + k], arg[ch * 8 + 2 * k], arg[ch * 8 + 2 * k + 1], P::mul(w[k], v2), jabs);
+    for (int k = 0; k < 4; k++) {
+      const uint32_t p = P::mul(w[k], v2);
+      const uint32_t m = P::template better<MAX>(p, pacc[ch * 4 + k]);
+      if (m & 0xffffu) arg[ch * 8 + 2 * k] = jabs;
+      if (m >> 16) arg[ch * 8 + 2 * k + 1] = jabs;
+      pacc[ch * 4 + k] = (p & m) | (pacc[ch * 4 + k] & ~m);
+    }
   }
 
   __device__ __forceinline__ void accumulate(IndexRing<T>& ring, int s, int e,
@@ -971,15 +983,11 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
 template <typename T, int RED, bool ACC = false, bool PLAN = false> static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(T);
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row
-  {  // narrow rows: group-per-row kernel (all reductions)
-    if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, 5, true, PLAN>(p, st);
-    if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, 5, true, PLAN>(p, st);
-    if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, 5, true, PLAN>(p, st);
-    if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, 5, true, PLAN>(p, st);
-  }
-  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 1, 6, false, PLAN>(p, st);
-  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, 5, false, PLAN>(p, st);
-  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, 5, false, PLAN>(p, st);
+  // narrow rows: group-per-row kernel (all reductions)
+  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, 5, true, PLAN>(p, st);
+  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, 5, true, PLAN>(p, st);
+  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, 5, true, PLAN>(p, st);
+  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, 5, true, PLAN>(p, st);
   // 256-byte rows (F = 128 bf16): at MINB = 5 the 48-register budget spills (120 B of stack in the planned kernel);
   // 3 CTAs/SM with 6 gathers in flight per lane is 8 % faster at C2 on the H100 (sweep in DESIGN §3.1)
   if (vecs <= 16) return launch_vec<T, RED, ACC, 16, 1, 6, 3, false, PLAN>(p, st);

@@ -148,7 +148,11 @@ def spmm_fw(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor,
             reduce: str, plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor]]:
     """`spmm_fw(rowptr, col, optional_value, mat, reduce) -> (out, arg_out?)`
     (csrc/spmm.cpp:22-35; checks follow csrc/cuda/spmm_cuda.cu:97-110). With a `plan` (spmm_plan(rowptr, E)) the
-    product is one memset + one kernel (tsb200_spmm_fw_planned); results are the same."""
+    product is one memset + one kernel (tsb200_spmm_fw_planned). min/max results and arg_out are the same as without
+    a plan, and so are sums over dense rows wider than 128 bytes. For narrower rows a sum can differ in the last bits
+    (within the same rounding bound) on rows the plan defers for the nnz budget of their 32-row group, when the
+    unplanned call uses smaller work items (matrices of fewer than about 500k rows): such a row is summed by several
+    lane groups instead of one."""
     _check_cuda(rowptr, "rowptr")
     _check_cuda(col, "col")
     if value is not None:

@@ -87,7 +87,8 @@ def test_random_shapes(oracle, shape, dtype, reduce):
 @pytest.mark.parametrize("dtype,reduce", list(product([torch.float32, torch.bfloat16], REDUCES)))
 def test_long_rows_and_budget(oracle, dtype, reduce):
     """rows longer than the 256-nnz segment length (multi-segment combine), a row of exactly 256/257,
-    and a dense 32-row block that exceeds the 1024-nnz item budget (single-segment deferral)."""
+    and a dense 32-row block that exceeds the 1024-nnz item budget. At M = 200 the work items are single rows, so
+    the budget does not defer anything here; test_spmm_kernels_gpu.py runs it with full-size items."""
     M, N, K = 200, 1500, 64
     long_rows = [(5, 1400), (6, 256), (7, 257), (100, 700)] + [(r, 60) for r in range(128, 160)]
     row, rowptr, col = random_csr(M, N, 4, seed=3, empty_rows=(0, 8, 199), long_rows=long_rows)

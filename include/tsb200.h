@@ -185,6 +185,8 @@ TSB200_API int tsb200_csr2csc(const int64_t* row, const int64_t* col, int64_t E,
  *   ptr i64[S+1]; perm i64[E] or NULL; value dtype[E, D]; out dtype[S, D]; reduce in {SUM, MEAN, MIN, MAX}.
  *   arg_out i64[S, D] (optional, MIN/MAX only): INPUT position (perm applied) of the first entry of the segment that
  *   attains the extreme (strict compare, like csrc/cpu/reducer.h:57-70), -1 for an empty segment.
+ *   SUM/MEAN start at +0 (torch_scatter's reducer does): a segment of -0 entries gives +0. MIN/MAX compare strictly
+ *   from the segment's first entry: a NaN there is the result (arg = that entry), a NaN anywhere else never is.
  * ------------------------------------------------------------------------------------------ */
 TSB200_API int tsb200_segment_reduce(const int64_t* ptr, const int64_t* perm, const void* value, void* out,
                                      int64_t* arg_out, int64_t S, int64_t D, int dtype, int reduce, void* stream);
@@ -217,6 +219,10 @@ TSB200_API int tsb200_segment_reduce_bw(const int64_t* seg, const int64_t* count
  *     position of the first entry of each run. For the backward of the value reduction (tsb200_segment_reduce_bw)
  *     the call can also emit seg_out i64[E] (run id of every INPUT entry), count_out i64[E'] (run lengths) and
  *     arg_out i64[E', D] (MIN/MAX: input position of the earliest entry attaining the extreme); each may be NULL.
+ *     Same rules as tsb200_segment_reduce: SUM/MEAN start at +0 (a run of -0 gives +0); MIN/MAX compare strictly
+ *     from the run's first entry (a NaN there is the result, a NaN later in the run never is).
+ *   The key is one 64-bit word: tsb200_coalesce_sort returns TSB200_ERR_UNSUPPORTED for M * N > 2^64 (and for
+ *   E >= 2^31).
  *   The same workspace must be passed to both phases.
  *   Synchronisation: phase 1 synchronises `stream` once internally (it reads back an "input already sorted"
  *   flag to skip the sort, like the reference's check at storage.py:154); phase 2 and tsb200_coalesce_perm

@@ -109,6 +109,8 @@ coalesce_emit_kernel(const uint64_t* __restrict__ k0, const uint64_t* __restrict
         else if (reduce == C_MIN) { if (v < a) { a = v; first = pj; } }   // strict: ties keep the earliest input entry
         else { if (v > a) { a = v; first = pj; } }
       }
+      // the sum starts at +0 (torch_scatter's does): x + 0 == x except that a run of -0 comes out +0
+      if (reduce == C_SUM || reduce == C_MEAN) a = a + (acc_t)0;
       if (reduce == C_MEAN) a = a / (acc_t)(e - s);
       value_out[seg * D + d] = Traits<T>::from_acc(a);
       if (arg_out) arg_out[seg * D + d] = first;
@@ -174,6 +176,9 @@ extern "C" int tsb200_coalesce_sort(const int64_t* row, const int64_t* col, int6
                                     void* stream) {
   if (E < 0 || M < 0 || N < 0) return TSB200_ERR_INVALID_ARG;
   if (E >= ((int64_t)1 << 31)) return TSB200_ERR_UNSUPPORTED;
+  // the key row*N + col is one 64-bit word: wider shapes would wrap it and merge distinct entries
+  const unsigned __int128 maxkey = (unsigned __int128)(M > 0 ? M : 1) * (unsigned __int128)(N > 0 ? N : 1);
+  if (maxkey > ((unsigned __int128)1 << 64)) return TSB200_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   const CoLayout L = co_layout(E);
   if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
@@ -190,10 +195,7 @@ extern "C" int tsb200_coalesce_sort(const int64_t* row, const int64_t* col, int6
   uint32_t* p0 = (uint32_t*)(ws + L.p0); uint32_t* p1 = (uint32_t*)(ws + L.p1);
   // key width and packing decision
   int bits = 1;
-  {
-    const unsigned __int128 maxkey = (unsigned __int128)(M > 0 ? M : 1) * (unsigned __int128)(N > 0 ? N : 1);
-    while (bits < 64 && ((unsigned __int128)1 << bits) < maxkey) bits++;
-  }
+  while (bits < 64 && ((unsigned __int128)1 << bits) < maxkey) bits++;
   int ebits = 1;
   while (((int64_t)1 << ebits) < E) ebits++;
   const int ib = (bits + ebits <= 64) ? ebits : 0;

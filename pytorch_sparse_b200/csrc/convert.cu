@@ -109,11 +109,22 @@ segment_reduce_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict
       // lanes goes to the smaller position, so the arg is the FIRST entry of the segment that attains the extreme
       // (torch_scatter's strict-compare rule, same as csrc/cpu/reducer.h:57-70 for SpMM)
       int64_t jpos = -1, asrc = -1;
-      for (int64_t j = b + lane; j < e; j += 32) {
+      int64_t j = b + lane;
+      // the lane's first entry starts its running value. Min/max compare strictly from the SEGMENT's first entry, so
+      // a NaN there wins and a NaN anywhere else never does: a lane skips a later NaN as its first entry (kept, no
+      // compare would ever replace it, and it would win the combine).
+      for (; j < e; j += 32) {
         const int64_t src = perm ? __ldg(perm + j) : j;
         const acc_t v = Traits<T>::to_acc(value[src * D + d]);
-        if (!have) { a = v; have = true; jpos = j; asrc = src; }
-        else if (reduce == TSB200_SUM || reduce == TSB200_MEAN) a = a + v;
+        if (v != v && j != b && (reduce == TSB200_MIN || reduce == TSB200_MAX)) continue;
+        a = v; have = true; jpos = j; asrc = src;
+        j += 32;
+        break;
+      }
+      for (; j < e; j += 32) {
+        const int64_t src = perm ? __ldg(perm + j) : j;
+        const acc_t v = Traits<T>::to_acc(value[src * D + d]);
+        if (reduce == TSB200_SUM || reduce == TSB200_MEAN) a = a + v;
         else if (reduce == TSB200_MIN) { if (v < a) { a = v; jpos = j; asrc = src; } }
         else { if (v > a) { a = v; jpos = j; asrc = src; } }
       }
@@ -131,6 +142,8 @@ segment_reduce_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict
         }
       }
       if (lane == 0) {
+        // the sum starts at +0 (torch_scatter's does): x + 0 == x except that a run of -0 comes out +0
+        if (reduce == TSB200_SUM || reduce == TSB200_MEAN) a = a + (acc_t)0;
         if (reduce == TSB200_MEAN && e > b) a = a / (acc_t)(e - b);
         out[seg * D + d] = Traits<T>::from_acc(have ? a : (acc_t)0);
         if (arg_out) arg_out[seg * D + d] = have ? asrc : (int64_t)-1;

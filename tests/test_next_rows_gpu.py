@@ -7,7 +7,7 @@ import torch
 
 import pytorch_sparse_b200 as ts
 from pytorch_sparse_b200 import ops
-from util import random_csr
+from util import assert_spspmm_values, random_csr, segment_sum_ref_bound
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -69,17 +69,14 @@ def test_segment_reduce_vs_oracle(oracle, dtype, reduce):
     g = torch.Generator().manual_seed(1)
     v = torch.randn(col.numel(), 2, generator=g)
     v = (v * 10).round().to(dtype) if dtype == torch.int64 else v.to(dtype)
-    out = ops.segment_reduce(rowptr.to(DEV), v.to(DEV), reduce)
-    ref = oracle.segment_reduce(rowptr, v, reduce)
-    if dtype == torch.int64 or reduce in ("min", "max"):
-        assert torch.equal(out.cpu(), ref)
-    else:  # warp-tree summation order differs from the sequential oracle
-        tol = 1e-5 if dtype == torch.float32 else 1e-12
-        assert torch.allclose(out.cpu(), ref, rtol=tol, atol=tol * 50)
     perm = torch.randperm(col.numel(), generator=g)
-    out_p = ops.segment_reduce(rowptr.to(DEV), v.to(DEV), reduce, perm=perm.to(DEV))
-    ref_p = oracle.segment_reduce(rowptr, v, reduce, perm=perm)
-    assert torch.allclose(out_p.cpu().double(), ref_p.double(), rtol=1e-5, atol=1e-3)
+    for p in (None, perm):
+        out = ops.segment_reduce(rowptr.to(DEV), v.to(DEV), reduce, perm=None if p is None else p.to(DEV)).cpu()
+        if dtype == torch.int64 or reduce in ("min", "max"):
+            assert torch.equal(out, oracle.segment_reduce(rowptr, v, reduce, perm=p))
+        else:  # warp-tree summation order differs from the sequential oracle: the rounding bound
+            ref, bound = segment_sum_ref_bound(oracle, rowptr, v, p, mean=reduce == "mean")
+            assert_spspmm_values(out, ref, bound, f"{dtype} {reduce} perm={p is not None}")
 
 
 def test_mul_vs_reference_and_gcn_flow():

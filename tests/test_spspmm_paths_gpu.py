@@ -616,13 +616,13 @@ def test_auto_mode_kernels(monkeypatch, dtype):
     va, vb = randn_values(case.nnz_a, dtype, 1).to(DEV), randn_values(case.nnz_b, dtype, 2).to(DEV)
     T = "float" if dtype == torch.float32 else "double"
 
-    def kernels(mode):
+    def kernels(mode, patterns):
         monkeypatch.setenv("TSB200_SPSPMM", mode)
         names = launched_kernels(lambda: ops.spspmm(rpa, ca, va, rpb, cb, vb, case.M, case.Kd, case.N, True),
-                                 r"spspmm_kernel<")
+                                 patterns)
         return {m.groups() for n in names for m in [re.search(r"spspmm_kernel<(\d), (float|double)>", n)] if m}, names
 
-    got, names = kernels("auto")
+    got, names = kernels("auto", [r"spspmm_kernel<"])
     assert got == {("2", T)}, names
-    got, names = kernels("two_phase")
+    got, names = kernels("two_phase", [r"spspmm_kernel<0,", r"spspmm_kernel<1,"])
     assert got == {("0", "float"), ("1", T)}, names

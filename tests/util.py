@@ -94,11 +94,37 @@ def assert_spspmm_values(v, ref, bound, what="", where=None):
                              + (f"; {where(~ok)}" if where else ""))
 
 
+_STORE_U = {torch.bfloat16: (2.0 ** -8, 2.0 ** -134), torch.float16: (2.0 ** -11, 2.0 ** -25)}
+
+
+def segment_sum_ref_bound(oracle, ptr, value, perm=None, mean=False):
+    """Reference values of a segment sum (or mean) and the per-entry error bound of a kernel that adds the segment's
+    n entries in any order in its accumulator (fp32 for fp32 / bf16 / f16, fp64 for fp64), divides once for the mean
+    and rounds once to the storage dtype. Against the oracle in fp64 on the values widened, with S = sum |v|:
+      sum : (n + 1) 2^-24 S (fp32 accumulator) or 2 (n + 1) 2^-53 S (fp64)
+      mean: (n + 2) u S / n (one more rounding, by the division)
+      bf16 / f16: plus 1/2 ulp of the storage dtype (relative 2^-8 / 2^-11 of the result, or half its smallest
+      subnormal). Entries with S = 0 (empty segments, all-zero segments) must be exactly +0."""
+    ptr, v = ptr.cpu(), value.cpu().double()
+    op = "mean" if mean else "sum"
+    ref = oracle.segment_reduce(ptr, v, op, perm=perm)
+    S = oracle.segment_reduce(ptr, v.abs(), "sum", perm=perm)
+    n = (ptr[1:] - ptr[:-1]).double().view((-1,) + (1,) * (v.dim() - 1))
+    u = 2.0 * 2.0 ** -53 if value.dtype == torch.float64 else 2.0 ** -24
+    bound = ((n + 2) * u * S / n.clamp(min=1)) if mean else ((n + 1) * u * S)
+    if value.dtype in _STORE_U:
+        rel, sub = _STORE_U[value.dtype]
+        bound = bound + torch.where(S > 0, rel * (ref.abs() + bound) + sub, torch.zeros_like(S))
+    return ref, bound
+
+
 def launched_kernels(fn, pattern=None):
     """Names of the kernels `fn` launches. A profiling session that delivers no kernel record at all, or none whose
-    name matches the regular expression `pattern`, is repeated: every call profiled here launches such a kernel."""
+    name matches the regular expression `pattern` (with a list of expressions: none for one of them), is repeated:
+    every call profiled here launches such kernels, and the profiler now and then drops a record."""
     import re
     from torch.profiler import ProfilerActivity, profile
+    patterns = [] if pattern is None else [pattern] if isinstance(pattern, str) else list(pattern)
     names = []
     for _ in range(3):
         torch.cuda.synchronize()
@@ -106,6 +132,6 @@ def launched_kernels(fn, pattern=None):
             fn()
             torch.cuda.synchronize()
         names = [e.name for e in prof.events() if "kernel" in e.name]
-        if names and (pattern is None or any(re.search(pattern, n) for n in names)):
+        if names and all(any(re.search(p, n) for n in names) for p in patterns):
             return names
     raise AssertionError(f"the profiler recorded no kernel{'' if pattern is None else ' matching ' + pattern}: {names}")

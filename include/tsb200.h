@@ -116,6 +116,25 @@ TSB200_API int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
                                       int64_t n_long, int64_t n_slot, void* workspace, size_t workspace_bytes,
                                       void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * SpMM over an FP8 (e4m3) dense operand (no counterpart in the reference).  B = 1.
+ *   out[m,:] = reduce_{e in row m} w_e * x8[col[e], :]   with   w_e = fl32(value[e] * scale[col[e] * scale_stride])
+ *   x8 e4m3[N, K] (K % 16 == 0, 16-byte aligned), scale f32 (scale_stride 0: one scale for the whole operand, 1: one
+ *   per dense row), value out_dtype[E] or NULL (1), out out_dtype[M, K] with out_dtype in {F32, F16, BF16},
+ *   arg_out i64[M, K] for MIN/MAX. x8 elements widen to fp32 exactly. SUM/MEAN: fp32 FFMA of w_e * x8 over the row,
+ *   MEAN divides by max(deg, 1), one rounding to out_dtype. MIN/MAX: strict compare of p = round_out(fl32(w_e * x8)),
+ *   the smallest e wins ties, out = p; empty rows, NaN and +-0 as tsb200_spmm_fw.
+ *   plan == NULL: unplanned, workspace tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce). Otherwise
+ *   `plan` is a tsb200_spmm_plan of rowptr with its counts, workspace tsb200_spmm_fw_planned_workspace_bytes(K,
+ *   n_long, n_slot, reduce); results as tsb200_spmm_fw_planned vs tsb200_spmm_fw. TSB200_ERR_UNSUPPORTED for
+ *   K % 16 != 0, another out_dtype, or a misaligned pointer (x8 / out 16 B, col 8 B, value / scale 4 B, arg_out 16 B).
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                  const float* scale, int64_t scale_stride, void* out, int64_t* arg_out, int64_t M,
+                                  int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
+                                  size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
 /* One COLUMN BLOCK of a SUM SpMM (multi-GPU pipelining: the dense operand arrives block by block over NVLink and
  * block p of A's columns is multiplied as soon as block p of `mat` has landed; no counterpart in the reference, which
  * has no collectives — the partitioner semantics are torch_sparse/narrow.py:15-42). (rowptr, col, value) hold only the

@@ -56,6 +56,10 @@ struct SpmmParams {
   void* part_val;      // acc_t [slots, K]
   int64_t* part_arg;   // int64 [slots, K] (min/max)
   int64_t seg_cap, long_cap, slot_cap;
+  // fp8 dense operand (tsb200_spmm_fw_fp8): the weight of entry e is fl32(value[e] * scale[col[e] * scale_stride]),
+  // scale_stride 0 = one scale for the whole operand, 1 = one per dense row
+  const float* scale;
+  uint32_t scale_stride;
 };
 
 // ---- per-warp streaming index ring ------------------------------------------------------------
@@ -224,6 +228,26 @@ template <> struct Vec<__half> {
   // min/max compare on the product rounded to the storage type, as the reference does
   // (csrc/cpu/spmm_cpu.cpp:81-83 forms `val * mat` in scalar_t).
   static __device__ __forceinline__ float round_prod(float x) { return __half2float(__float2half_rn(x)); }
+};
+// e4m3 dense operand: a 16-byte gather is 16 elements, widened pairwise through f16x2 (cvt.rn.f16x2.e4m3x2, sm_89+)
+// and then to fp32; both steps are exact (every e4m3 value, NaN included, is an f16 value). Only the unpack is used:
+// values and outputs keep their own type (Vec<T> above).
+template <> struct Vec<__nv_fp8_e4m3> {
+  static constexpr int VEC = 16;
+  static __device__ __forceinline__ void unpack(const uint4& d, float* f) {
+    const uint32_t w[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        uint32_t r;
+        asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)(w[i] >> (16 * h))));
+        const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&r));
+        f[4 * i + 2 * h] = t.x;
+        f[4 * i + 2 * h + 1] = t.y;
+      }
+    }
+  }
 };
 
 

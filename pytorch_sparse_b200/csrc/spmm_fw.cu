@@ -19,6 +19,8 @@
 //     item's nnz budget are deferred into a device-side segment queue (<= SEG nnz each); a
 //     second kernel runs one warp per segment, a third combines multi-segment rows in
 //     segment order (deterministic; min/max keep the smallest-e tie-break).
+//   * the dense operand may be FP8 (e4m3, tsb200_spmm_fw_fp8): the same kernels with the dense type X split from the
+//     value / output type T; 16 columns per 128-bit gather, each entry weighted by value * scale[col], fp32 min/max;
 //   * anything the vector path cannot take (K*sizeof(T) % 16 != 0, integer / fp64 types,
 //     unaligned pointers, E >= 2^31) goes to a generic lane-per-column kernel that walks the
 //     nnz sequentially exactly like csrc/cpu/spmm_cpu.cpp:75-88 (bit-identical for fp32/fp64).
@@ -26,15 +28,20 @@
 
 namespace tsb {
 
-template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
+// T = value / output type, X = dense-operand type: T itself, or __nv_fp8_e4m3 (tsb200_spmm_fw_fp8), in which case
+// every entry's weight is fl32(value * scale[col]) and a 16-byte gather carries 16 columns.
+template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct RowEngine {
   using V = Vec<T>;
-  static constexpr int VEC = V::VEC;
+  static constexpr bool Q8 = !std::is_same<X, T>::value;
+  static constexpr int VEC = Vec<X>::VEC;
   static constexpr int G = 32 / LPR;
   static constexpr int NA = VEC * CH;
   static constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
 
   float acc[NA];
   int arg[ARG ? NA : 1];
+  const float* scale;  // Q8 only
+  uint32_t sstride;
 
   __device__ __forceinline__ float acc_float(int i) const { return acc[i]; }
 
@@ -51,11 +58,10 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
     }
   }
 
-  // one step of the min/max update (compare on the product rounded to the storage type)
-  __device__ __forceinline__ void minmax_step(float* a, int* ar, typename V::vraw v, const uint4& d, int jabs) {
+  // one step of the min/max update (compare on the product rounded to the storage type); vf = the entry's weight
+  __device__ __forceinline__ void minmax_step(float* a, int* ar, float vf, const uint4& d, int jabs) {
     float f[VEC];
-    V::unpack(d, f);
-    const float vf = V::vfloat(v);
+    Vec<X>::unpack(d, f);
 #pragma unroll
     for (int i = 0; i < VEC; i++) {
       const float p = V::round_prod(vf * f[i]);  // v == 1 when has_value=false => p == f
@@ -64,6 +70,26 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
         a[i] = p;
         ar[i] = jabs;
       }
+    }
+  }
+
+  // scale of the dense row an entry gathers (fp8 operand); stride 0 reads one value for the whole operand
+  __device__ __forceinline__ float row_scale(uint32_t c) const { return __ldg(scale + (size_t)c * sstride); }
+
+  // one gathered vector of one entry: v = raw value, s = its dense row's scale (Q8), d = the 16 bytes
+  __device__ __forceinline__ void step(int ch, typename V::vraw v, float s, const uint4& d, int jabs) {
+    if constexpr (RED == R_SUM) {
+      if constexpr (Q8) {
+        const float w = V::vfloat(v) * s;
+        float f[VEC];
+        Vec<X>::unpack(d, f);
+#pragma unroll
+        for (int i = 0; i < VEC; i++) acc[ch * VEC + i] = fmaf(w, f[i], acc[ch * VEC + i]);
+      } else {
+        V::fma(&acc[ch * VEC], v, d);
+      }
+    } else {
+      minmax_step(&acc[ch * VEC], &arg[ch * VEC], Q8 ? V::vfloat(v) * s : V::vfloat(v), d, jabs);
     }
   }
 
@@ -86,6 +112,7 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
       const int jabs0 = (int)ring.base + j0 + g;  // absolute nnz index of step 0 (E < 2^31)
       uint4 d[U][CH];
       VR v[U];
+      float sc[U];
       if (jend - j0 == U * G) {  // full chunk: every lane group has work in every step
 #pragma unroll
         for (int u = 0; u < U; u++) {
@@ -95,14 +122,14 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
 #pragma unroll
           for (int ch = 0; ch < CH; ch++)
             if (col_ok[ch]) d[u][ch] = ldg128_hint(src + ch * (LPR * 16), pol);
+          if constexpr (Q8) sc[u] = row_scale(c);
         }
 #pragma unroll
         for (int u = 0; u < U; u++) {
 #pragma unroll
           for (int ch = 0; ch < CH; ch++) {
             if (!col_ok[ch]) continue;
-            if (RED == R_SUM) V::fma(&acc[ch * VEC], v[u], d[u][ch]);
-            else minmax_step(&acc[ch * VEC], &arg[ch * VEC], v[u], d[u][ch], jabs0 + u * G);
+            step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
           }
         }
       } else {
@@ -119,6 +146,7 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
 #pragma unroll
           for (int ch = 0; ch < CH; ch++)
             if (act[u] && col_ok[ch]) d[u][ch] = ldg128_hint(src + ch * (LPR * 16), pol);
+          if constexpr (Q8) sc[u] = act[u] ? row_scale(c) : 0.f;
         }
 #pragma unroll
         for (int u = 0; u < U; u++) {
@@ -126,8 +154,7 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
 #pragma unroll
           for (int ch = 0; ch < CH; ch++) {
             if (!(act[u] && col_ok[ch])) continue;
-            if (RED == R_SUM) V::fma(&acc[ch * VEC], v[u], d[u][ch]);
-            else minmax_step(&acc[ch * VEC], &arg[ch * VEC], v[u], d[u][ch], jabs0 + u * G);
+            step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
           }
         }
       }
@@ -186,7 +213,8 @@ template <typename T, int RED, int LPR, int CH, int U> struct RowEngine {
           continue;
         }
       }
-      stg128_stream(out_row + koff, V::pack(f));
+#pragma unroll
+      for (int i = 0; i < VEC; i += V::VEC) stg128_stream(out_row + koff + i, V::pack(f + i));  // 2-4 stores for Q8
       if (ARG) {
 #pragma unroll
         for (int i = 0; i < VEC; i += 2) {
@@ -271,6 +299,7 @@ template <> struct Pk<__half> {
 template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
   using V = Vec<T>;
   using P = Pk<T>;
+  static constexpr bool Q8 = false;
   static constexpr int VEC = 8;
   static constexpr int G = 32 / LPR;
   static constexpr int NA = VEC * CH;
@@ -379,10 +408,17 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
   }
 };
 
-template <typename T, int RED, int LPR, int CH, int U> struct EngineFor {
-  using type = typename std::conditional<(RED != R_SUM && is_float16<T>::value), MinMax16Engine<T, RED, LPR, CH, U>,
-                                         RowEngine<T, RED, LPR, CH, U>>::type;
+// min/max over an fp8 operand compare in fp32 (the packed engine multiplies two values of the storage type)
+template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct EngineFor {
+  using type = typename std::conditional<(RED != R_SUM && is_float16<T>::value && std::is_same<X, T>::value),
+                                         MinMax16Engine<T, RED, LPR, CH, U>, RowEngine<T, RED, LPR, CH, U, X>>::type;
 };
+template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, const SpmmParams& p) {
+  if constexpr (Eng::Q8) {
+    eng.scale = p.scale;
+    eng.sstride = p.scale_stride;
+  }
+}
 
 // combine the partials of one multi-segment row, in segment order, by ONE WARP (planned mode: the warp that finished
 // the row's last segment); the partials were written by other SMs -> read them past L1
@@ -411,10 +447,10 @@ __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const Long
   }
 }
 
-template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false>
+template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_vec_kernel(const SpmmParams p) {
-  using Eng = typename EngineFor<T, RED, LPR, CH, U>::type;
+  using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
@@ -439,8 +475,8 @@ spmm_vec_kernel(const SpmmParams p) {
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
-  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(T);
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
+  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
 
   const int item_rows = 1 << p.item_shift;
   const int64_t nblk = (p.M + item_rows - 1) >> p.item_shift;
@@ -522,6 +558,7 @@ spmm_vec_kernel(const SpmmParams p) {
       const int e = __shfl_sync(0xffffffffu, e_rel, rl);
       Eng eng;
       eng.init();
+      set_scale(eng, p);
       eng.accumulate(ring, s, e, matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
       if (g == 0) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
@@ -548,6 +585,7 @@ spmm_vec_kernel(const SpmmParams p) {
       asm volatile("" : "+l"(matb));
       Eng eng;
       eng.init();
+      set_scale(eng, p);
       eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
       if (S.slot < 0) {
@@ -601,19 +639,20 @@ template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __
   return __ldg(reinterpret_cast<const unsigned short*>(p));
 }
 
-template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false>
+template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_gpr_kernel(const SpmmParams p) {
   using V = Vec<T>;
-  using Eng = typename EngineFor<T, RED, LPR, 1, U>::type;  // per-lane state + update + store of one row
+  using Eng = typename EngineFor<T, RED, LPR, 1, U, X>::type;  // per-lane state + update + store of one row
   using VR = typename V::vraw;
-  constexpr int VEC = V::VEC;
+  constexpr int VEC = Eng::VEC;
+  constexpr bool Q8 = Eng::Q8;
   constexpr int G = 32 / LPR;
   const int lane = threadIdx.x & 31;
   const int g = lane / LPR, li = lane % LPR;
   const bool col_ok = p.k0 + li * VEC < p.K;
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
-  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(T);
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
+  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
   const uint64_t pol = make_policy_evict_last();
   const T* __restrict__ val = (const T*)p.value;
   const bool has_val = val != nullptr;
@@ -706,6 +745,7 @@ spmm_gpr_kernel(const SpmmParams p) {
 
       Eng eng;
       eng.init();
+      set_scale(eng, p);
 
       // software pipeline: the (col, value) pairs of chunk k+1 are loaded while chunk k's gathers fly
       uint32_t cn[U];
@@ -722,12 +762,14 @@ spmm_gpr_kernel(const SpmmParams p) {
       for (int j0 = 0; j0 < maxlen; j0 += U) {
         uint4 d[U];
         VR v[U];
+        float sc[U];
         bool act[U];
 #pragma unroll
         for (int u = 0; u < U; u++) {
           act[u] = (j0 + u < len) && col_ok;
           v[u] = vn[u];
           if (act[u]) d[u] = ldg128_hint(matb + (uint64_t)cn[u] * row_bytes, pol);
+          if constexpr (Q8) sc[u] = act[u] ? eng.row_scale(cn[u]) : 0.f;
         }
 #pragma unroll
         for (int u = 0; u < U; u++) {
@@ -740,9 +782,10 @@ spmm_gpr_kernel(const SpmmParams p) {
 #pragma unroll
         for (int u = 0; u < U; u++) {
           if (!act[u]) continue;
-          if constexpr (RED == R_SUM) V::fma(eng.acc, v[u], d[u]);
+          if constexpr (Q8) eng.step(0, v[u], sc[u], d[u], jbase + s + j0 + u);
+          else if constexpr (RED == R_SUM) V::fma(eng.acc, v[u], d[u]);
           else if constexpr (is_float16<T>::value) eng.vec_step(0, v[u], d[u], jbase + s + j0 + u);
-          else eng.minmax_step(eng.acc, eng.arg, v[u], d[u], jbase + s + j0 + u);
+          else eng.minmax_step(eng.acc, eng.arg, V::vfloat(v[u]), d[u], jbase + s + j0 + u);
         }
       }
       if (mine) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
@@ -753,10 +796,10 @@ spmm_gpr_kernel(const SpmmParams p) {
 }
 
 // one warp per queued segment
-template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false>
+template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_seg_kernel(const SpmmParams p) {
-  using Eng = typename EngineFor<T, RED, LPR, CH, U>::type;
+  using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
@@ -780,8 +823,8 @@ spmm_seg_kernel(const SpmmParams p) {
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
-  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(T);
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
+  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
 
   const int64_t nseg = p.plan_mask ? p.n_seg : min((int64_t)p.counters[1], p.seg_cap);
   const int64_t wstride = (int64_t)gridDim.x * kWarpsPerCta;
@@ -794,6 +837,7 @@ spmm_seg_kernel(const SpmmParams p) {
     asm volatile("" : "+l"(matb));
     Eng eng;
     eng.init();
+    set_scale(eng, p);
     eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
     eng.reduce_groups();
     if (g == 0) {
@@ -924,15 +968,16 @@ static bool vec_eligible(int dtype, int64_t K, int64_t E, int64_t N, const void*
   return true;
 }
 
-template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false>
+template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false,
+          typename X = T>
 static int launch_vec(SpmmParams p, cudaStream_t st) {
-  constexpr int VEC = 16 / sizeof(T);
+  constexpr int VEC = 16 / sizeof(X);
   constexpr int kcols = LPR * CH * VEC;
   void (*kmain)(const SpmmParams);
-  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN>;
-  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN>;
+  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X>;
+  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X>;
   constexpr int USEG = (U > LPR) ? LPR : U;  // the row engine needs U * (32 / LPR) <= 32
-  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC>;
+  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   // small matrices: shrink the work item so that every resident warp gets rows
@@ -980,29 +1025,38 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
 // (LPR, CH) follow from the width of a dense row; (U, MINB) = gathers in flight per lane and CTAs
 // per SM: the kernel is HBM-latency bound, so resident warps x gathers-in-flight wins (40 warps/SM x 4 x 16 B
 // per lane; the register budget of MINB = 5 is the same 64K registers per SM on sm_90).
-template <typename T, int RED, bool ACC = false, bool PLAN = false> static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
-  constexpr int VEC = 16 / sizeof(T);
+template <typename T, int RED, bool ACC = false, bool PLAN = false, typename X = T>
+static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
+  // fp8 operand: a vector is 16 columns, so a lane keeps twice the accumulators (and arg slots) of a 16-bit operand
+  // and needs more registers per thread: its own (U, CTAs/SM) per shape (ptxas report and times in DESIGN §3.1)
+  constexpr bool Q8 = !std::is_same<X, T>::value;
+  constexpr bool MM = RED != R_SUM;
+  constexpr int VEC = 16 / sizeof(X);
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row
   // narrow rows: group-per-row kernel (all reductions)
-  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, 5, true, PLAN>(p, st);
-  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, 5, true, PLAN>(p, st);
-  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, 5, true, PLAN>(p, st);
-  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, 5, true, PLAN>(p, st);
+  constexpr int GB = Q8 ? (MM ? 2 : 3) : 5;
+  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X>(p, st);
+  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X>(p, st);
+  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X>(p, st);
+  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, GB, true, PLAN, X>(p, st);
   // 256-byte rows (F = 128 bf16): at MINB = 5 the 48-register budget spills (120 B of stack in the planned kernel);
   // 3 CTAs/SM with 6 gathers in flight per lane is 8 % faster at C2 on the H100 (sweep in DESIGN §3.1)
-  if (vecs <= 16) return launch_vec<T, RED, ACC, 16, 1, 6, 3, false, PLAN>(p, st);
-  if (vecs <= 32) return launch_vec<T, RED, ACC, 32, 1, 4, 5, false, PLAN>(p, st);
-  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, 4, 3, false, PLAN>(p, st);
-  return launch_vec<T, RED, ACC, 32, 4, 2, 3, false, PLAN>(p, st);  // column-tiled beyond 128 vectors
+  if (vecs <= 16)
+    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && MM ? 2 : 3, false, PLAN, X>(p, st);
+  if (vecs <= 32) return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (MM ? 2 : 3) : 5, false, PLAN, X>(p, st);
+  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X>(p, st);
+  // column-tiled beyond 128 vectors
+  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (MM ? 1 : 2) : 3, false, PLAN, X>(p, st);
 }
 
-template <typename T, bool PLAN = false> static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
+template <typename T, bool PLAN = false, typename X = T>
+static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
   p.mean = (reduce == TSB200_MEAN);
   switch (reduce) {
     case TSB200_SUM:
-    case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN>(p, st);
-    case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN>(p, st);
-    case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN>(p, st);
+    case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN, X>(p, st);
+    case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN, X>(p, st);
+    case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN, X>(p, st);
   }
   return TSB200_ERR_INVALID_ARG;
 }
@@ -1288,6 +1342,81 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
     case TSB200_F32: return dispatch_red_vec<float, true>(p, reduce, st);
     case TSB200_F16: return dispatch_red_vec<__half, true>(p, reduce, st);
     case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, true>(p, reduce, st);
+  }
+  return TSB200_ERR_UNSUPPORTED;
+}
+
+// ---- SpMM over an fp8 (e4m3) dense operand with per-tensor or per-row scales ----------------------------------------
+// The same kernels, instantiated with X = __nv_fp8_e4m3: value / output type T = out_dtype, a dense row is K bytes.
+extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                  const float* scale, int64_t scale_stride, void* out, int64_t* arg_out, int64_t M,
+                                  int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
+                                  size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
+  if (reduce < TSB200_SUM || reduce > TSB200_MAX) return TSB200_ERR_INVALID_ARG;
+  if (scale_stride != 0 && scale_stride != 1) return TSB200_ERR_INVALID_ARG;
+  if (out_dtype != TSB200_F32 && out_dtype != TSB200_F16 && out_dtype != TSB200_BF16) return TSB200_ERR_UNSUPPORTED;
+  if (K % 16 != 0) return TSB200_ERR_UNSUPPORTED;
+  const bool arg = (reduce == TSB200_MIN || reduce == TSB200_MAX);
+  if (M * K == 0) return 0;
+  if (!rowptr || !out || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (E == 0) {  // every row is empty: 0, and arg_out = E = 0
+    TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(M * K) * dtype_size(out_dtype), st));
+    if (arg) TSB_CUDA_TRY(cudaMemsetAsync(arg_out, 0, (size_t)(M * K) * sizeof(int64_t), st));
+    return 0;
+  }
+  if (!col || !mat || !scale) return TSB200_ERR_INVALID_ARG;
+  if (E >= ((int64_t)1 << 31) - 64 || N >= ((int64_t)1 << 32) || K >= ((int64_t)1 << 31)) return TSB200_ERR_UNSUPPORTED;
+  if (((uintptr_t)mat & 15) || ((uintptr_t)out & 15) || ((uintptr_t)col & 7) || ((uintptr_t)scale & 3))
+    return TSB200_ERR_UNSUPPORTED;
+  if ((value && ((uintptr_t)value & 3)) || (arg_out && ((uintptr_t)arg_out & 15))) return TSB200_ERR_UNSUPPORTED;
+  if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
+  char* ws = (char*)workspace;
+  SpmmParams p;
+  p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
+  p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
+  p.partial = nullptr; p.acc_mode = 0;
+  p.scale = scale; p.scale_stride = (uint32_t)scale_stride;
+  if (plan) {  // planned: the layout of tsb200_spmm_fw_planned
+    const PlanLayout PL = plan_layout(M, E);
+    if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
+    if (n_seg > PL.seg_cap || n_long > PL.long_cap || ((uintptr_t)plan & 255)) return TSB200_ERR_INVALID_ARG;
+    const PlannedWs W = planned_ws(K, n_long, n_slot, arg);
+    if (workspace_bytes < W.total) return TSB200_ERR_WORKSPACE;
+    const char* pl = (const char*)plan;
+    p.counters = (unsigned int*)(ws + W.counters);
+    p.long_done = (uint32_t*)(ws + W.long_done);
+    p.segs = (Segment*)(pl + PL.segs);
+    p.longs = (LongRow*)(pl + PL.longs);
+    p.seg_lr = (const uint32_t*)(pl + PL.seg_lr);
+    p.plan_mask = (const uint32_t*)(pl + PL.mask);
+    p.n_seg = n_seg; p.n_long = n_long;
+    p.part_val = ws + W.part_val;
+    p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
+    p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
+    switch (out_dtype) {
+      case TSB200_F32: return dispatch_red_vec<float, true, __nv_fp8_e4m3>(p, reduce, st);
+      case TSB200_F16: return dispatch_red_vec<__half, true, __nv_fp8_e4m3>(p, reduce, st);
+      case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, true, __nv_fp8_e4m3>(p, reduce, st);
+    }
+    return TSB200_ERR_UNSUPPORTED;
+  }
+  // unplanned: the layout of tsb200_spmm_fw (tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce))
+  const WsLayout L = ws_layout(1, K, E, arg);
+  if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
+  p.counters = (unsigned int*)(ws + L.counters);
+  p.segs = (Segment*)(ws + L.segs);
+  p.longs = (LongRow*)(ws + L.longs);
+  p.part_val = ws + L.part_val;
+  p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
+  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+  switch (out_dtype) {
+    case TSB200_F32: return dispatch_red_vec<float, false, __nv_fp8_e4m3>(p, reduce, st);
+    case TSB200_F16: return dispatch_red_vec<__half, false, __nv_fp8_e4m3>(p, reduce, st);
+    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, false, __nv_fp8_e4m3>(p, reduce, st);
   }
   return TSB200_ERR_UNSUPPORTED;
 }

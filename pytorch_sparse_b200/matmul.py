@@ -80,6 +80,35 @@ def spmm(src: SparseTensor, other: Tensor, reduce: str = "sum") -> Tensor:
         raise ValueError("unknown reduce '" + reduce + "'")
 
 
+def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
+             out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
+    """`src @ (x8 * scale)` over an FP8 (e4m3) dense operand `x8` [N, K] (K % 16 == 0) with a float32 `scale` of
+    shape [] or [N] (see `quantize_fp8`), reduce in sum/add/mean/min/max, result in `out_dtype` (bf16, f16, f32).
+    The entry values are cast to `out_dtype` first, as `spmm` casts them to the dense dtype. Forward only: no
+    gradient flows, and a `value` or `scale` that requires grad is refused while grad mode is on."""
+    rowptr, col, value = src.csr()
+    if value is not None:
+        value = value.to(out_dtype)
+    if reduce == "add":
+        reduce = "sum"
+    if reduce != "sum" and reduce != "mean" and reduce != "min" and reduce != "max":
+        raise ValueError("unknown reduce '" + reduce + "'")
+    return torch.ops.tsb200.spmm_fp8(rowptr, col, value, x8, scale, reduce, out_dtype)[0]
+
+
+def quantize_fp8(x: Tensor, per_row: bool = True) -> Tuple[Tensor, Tensor]:
+    """A 2-D floating `x` [N, K] as `(x8, scale)` for `spmm_fp8`: scale = amax|x| / 448 (e4m3's largest finite value)
+    per row ([N]) or over the whole tensor ([]), 1 where that amax is 0, and x8 = e4m3(x / scale), rounded to
+    nearest. Pure torch, on the device of `x`."""
+    if x.dim() != 2:
+        raise ValueError("quantize_fp8 expects a 2-D tensor [N, K]")
+    xf = x.float()
+    amax = xf.abs().amax(dim=1) if per_row else xf.abs().amax()
+    scale = torch.where(amax > 0, amax / 448.0, torch.ones_like(amax))
+    x8 = (xf / (scale.unsqueeze(1) if per_row else scale)).to(torch.float8_e4m3fn)
+    return x8, scale
+
+
 def spspmm_sum(src: SparseTensor, other: SparseTensor) -> SparseTensor:
     M, Kd = src.sparse_sizes()
     Kb, N = other.sparse_sizes()
@@ -134,6 +163,8 @@ def matmul(src, other, reduce="sum"):  # noqa: F811
 
 
 SparseTensor.spmm = lambda self, other, reduce="sum": spmm(self, other, reduce)
+SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bfloat16: spmm_fp8(
+    self, x8, scale, reduce, out_dtype)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)
 SparseTensor.__matmul__ = lambda self, other: matmul(self, other, "sum")

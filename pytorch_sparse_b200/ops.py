@@ -209,6 +209,87 @@ def spmm_fw(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor,
     return out, arg_out
 
 
+_FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
+
+
+def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
+                reduce: str = "sum", out_dtype: torch.dtype = torch.bfloat16,
+                plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor]]:
+    """`spmm_fw_fp8(rowptr, col, optional_value, x8, scale, reduce, out_dtype) -> (out, arg_out?)`
+    (tsb200_spmm_fw_fp8): the SpMM forward over an e4m3 dense operand `x8` [N, K] (K % 16 == 0) whose row c stands for
+    `x8[c].float() * scale[c]` (`scale` float32 of shape [N]) or `x8[c].float() * scale` (shape []). `value` has
+    `out_dtype` (bf16, f16 or f32), as `spmm_fw`'s value has the dense dtype. Entry e weighs fl32(value[e] * scale[c]);
+    sums accumulate weight * x8 in fp32 and round once, min/max compare the product rounded to `out_dtype`. Forward
+    only. Planned like `spmm_fw` (the same per-rowptr plan cache)."""
+    _check_cuda(rowptr, "rowptr")
+    _check_cuda(col, "col")
+    if value is not None:
+        _check_cuda(value, "optional_value.value()")
+    _check_cuda(x8, "x8")
+    _check_cuda(scale, "scale")
+    if torch.is_grad_enabled() and (scale.requires_grad or (value is not None and value.requires_grad)):
+        raise RuntimeError("spmm_fp8 is forward only: value and scale must not require grad "
+                           "(call it under torch.no_grad() or detach them)")
+    if x8.dtype != torch.float8_e4m3fn:
+        raise RuntimeError(f"spmm_fp8: x8 must be torch.float8_e4m3fn, got {x8.dtype}")
+    if x8.dim() != 2:
+        raise RuntimeError(f"spmm_fp8: x8 must be 2-D [N, K], got {x8.dim()}-D")
+    N, K = x8.shape
+    if K % 16 != 0:
+        raise RuntimeError(f"spmm_fp8: the number of columns K = {K} must be a multiple of 16")
+    if not x8.is_contiguous() or x8.data_ptr() % 16 != 0:
+        raise RuntimeError("spmm_fp8: x8 must be contiguous and 16-byte aligned")
+    if out_dtype not in _FP8_OUT:
+        raise RuntimeError(f"spmm_fp8: out_dtype must be torch.bfloat16, torch.float16 or torch.float32, got {out_dtype}")
+    if scale.dtype != torch.float32:
+        raise RuntimeError(f"spmm_fp8: scale must be float32, got {scale.dtype}")
+    if scale.dim() == 0:
+        stride = 0
+    elif scale.dim() == 1 and scale.size(0) == N:
+        stride = 1
+    else:
+        raise RuntimeError(f"spmm_fp8: scale must have shape [] or [N] = [{N}], got {list(scale.shape)}")
+    scale = scale.contiguous()
+    _check_input(rowptr.dim() == 1)
+    _check_input(col.dim() == 1)
+    if value is not None:
+        _check_input(value.dim() == 1)
+        _check_input(value.size(0) == col.size(0))
+        if value.dtype != out_dtype:
+            raise RuntimeError(f"expected value of dtype {out_dtype} but got {value.dtype}")
+        value = value.contiguous()
+    red = _reduce_code(reduce)
+    rowptr = _i64(rowptr, "rowptr")
+    col = _i64(col, "col")
+    M, E = rowptr.numel() - 1, col.numel()
+    dev = x8.device
+    out = torch.empty(M, K, dtype=out_dtype, device=dev)
+    arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
+    if out.numel() == 0:
+        return out, arg_out
+    if E == 0:
+        out.zero_()
+        if arg_out is not None:
+            arg_out.fill_(0)
+        return out, arg_out
+    with _on_device(dev):
+        if plan is None:
+            plan = _auto_plan(rowptr, E)
+        if plan is not None and (plan.M != M or plan.E != E):
+            plan = None
+        if plan is not None:
+            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
+            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
+        else:
+            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, _FP8_OUT[out_dtype], red)
+            pl, pl_bytes, counts = None, 0, (0, 0, 0)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_fw_fp8(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(out), _p(arg_out),
+                                     M, N, K, E, _FP8_OUT[out_dtype], red, pl, pl_bytes, *counts, _p(ws), nws,
+                                     _stream(dev)), "tsb200_spmm_fw_fp8")
+    return out, arg_out
+
+
 def spmm_fw_acc(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, partial: Tensor,
                 out: Optional[Tensor], acc_mode: int) -> None:
     """One column block of a SUM SpMM whose blocks are launched separately (tsb200_spmm_fw_acc): `partial` is the

@@ -2,7 +2,7 @@
 (csrc/spmm.cpp:305-348, csrc/convert.cpp:46-48):
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
-    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm}     (this package's own additions)
+    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8}   (this package's own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -43,6 +43,8 @@ _EXTRA_SCHEMAS = {
     "segment_reduce": "(Tensor ptr, Tensor value, str reduce, Tensor? perm, Tensor? seg) -> Tensor",
     "spspmm": "(Tensor rowptrA, Tensor colA, Tensor? valueA, Tensor rowptrB, Tensor colB, Tensor? valueB, "
               "int M, int K, int N, bool want_value) -> (Tensor, Tensor, Tensor, Tensor?)",
+    "spmm_fp8": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
+                "ScalarType out_dtype) -> (Tensor, Tensor?)",
 }
 
 
@@ -56,6 +58,8 @@ _EXTRA_IMPLS = {
     "coalesce": ops.coalesce, "sort_perm": ops.sort_perm, "csr2csc": _csr2csc,
     "segment_reduce": lambda ptr, value, reduce, perm, seg: ops.segment_reduce(ptr, value, reduce, perm, seg),
     "spspmm": ops.spspmm,
+    "spmm_fp8": lambda rowptr, col, value, x8, scale, reduce, out_dtype: ops.spmm_fw_fp8(rowptr, col, value, x8, scale,
+                                                                                         reduce, out_dtype),
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -135,6 +135,29 @@ TSB200_API int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, con
                                   size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
                                   size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * SpMM from an FP8 (e4m3) operand to an FP8 (e4m3) result with per-row scales, so that multi-hop propagation
+ * (X_{h+1} = A X_h) stays in e4m3 without a float copy of the hop (no counterpart in the reference).  B = 1.
+ *   Let y be the F32 result of tsb200_spmm_fw_fp8 with the same arguments and out_dtype = TSB200_F32, on the same path
+ *   (planned or unplanned; value f32[E] or NULL). Then, per row m:
+ *     out_scale[m] = amax_k |y[m,k]| / 448 (IEEE fp32 division, round to nearest), or 1 when that amax is not > 0
+ *                    (an all-zero or empty row, and a row holding NaN: the amax propagates NaN);
+ *     out8[m,k]    = e4m3(y[m,k] / out_scale[m]) (IEEE division), rounded to nearest even with subnormals kept, as
+ *                    torch's non-saturating float8_e4m3fn cast: |q| <= 464 rounds to at most 448, |q| > 464 and
+ *                    +-inf become NaN, -0 stays -0. An inf row gets scale inf: finite entries become +-0, inf NaN.
+ *   That is, bit for bit, torch's quantize_fp8(y, per_row=True) on the CPU. arg_out (MIN/MAX) is that call's arg_out.
+ *   out8 e4m3[M, K] (16-byte aligned), out_scale f32[M]: valid x8 / scale operands of the next hop.
+ *   Plan and workspace sizing as tsb200_spmm_fw_fp8 with out_dtype = TSB200_F32. E == 0: out8 = 0, out_scale = 1,
+ *   arg_out = 0. TSB200_ERR_UNSUPPORTED for K % 16 != 0, K > 2048 (one column tile: the row amax is not taken across
+ *   tiles), or a misaligned pointer (as tsb200_spmm_fw_fp8; out_scale 4 B).
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* col, const void* value,
+                                        const void* mat, const float* scale, int64_t scale_stride, void* out8,
+                                        float* out_scale, int64_t* arg_out, int64_t M, int64_t N, int64_t K,
+                                        int64_t E, int reduce, const void* plan, size_t plan_bytes, int64_t n_seg,
+                                        int64_t n_long, int64_t n_slot, void* workspace, size_t workspace_bytes,
+                                        void* stream);
+
 /* One COLUMN BLOCK of a SUM SpMM (multi-GPU pipelining: the dense operand arrives block by block over NVLink and
  * block p of A's columns is multiplied as soon as block p of `mat` has landed; no counterpart in the reference, which
  * has no collectives — the partitioner semantics are torch_sparse/narrow.py:15-42). (rowptr, col, value) hold only the

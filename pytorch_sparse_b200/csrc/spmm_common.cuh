@@ -60,6 +60,8 @@ struct SpmmParams {
   // scale_stride 0 = one scale for the whole operand, 1 = one per dense row
   const float* scale;
   uint32_t scale_stride;
+  // e4m3 result (tsb200_spmm_fw_fp8_quant): `out` is e4m3 [M, K], out_scale[m] = amax_k |y[m,k]| / 448 (1 if not > 0)
+  float* out_scale;
 };
 
 // ---- per-warp streaming index ring ------------------------------------------------------------
@@ -249,6 +251,35 @@ template <> struct Vec<__nv_fp8_e4m3> {
     }
   }
 };
+
+// ---- e4m3 result with a per-row scale (tsb200_spmm_fw_fp8_quant) ---------------------------------------------------
+// The definition is torch's quantize_fp8 on the CPU: s = amax|y| / 448 (IEEE division), 1 when amax is not > 0, then
+// e4m3(y / s). The amax keeps NaN (torch's amax propagates it; fmaxf would drop it), so a row holding NaN gets s = 1.
+__device__ __forceinline__ float amax_nan(float m, float a) { return (a > m || a != a) ? a : m; }
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f; }
+
+// two floats as e4m3 (lo in the low byte), following torch's non-saturating float8_e4m3fn cast: round to nearest even,
+// subnormals kept, -0 stays -0, and a magnitude past 464 (the midpoint above 448) or an inf becomes NaN.
+// cvt.rn.satfinite clamps those to +-448, so they are patched afterwards.
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  unsigned short r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  uint32_t w = r;
+  if (fabsf(lo) > 464.f) w = (w & 0xff00u) | 0x7fu;
+  if (fabsf(hi) > 464.f) w = (w & 0x00ffu) | 0x7f00u;
+  return w;
+}
+__device__ __forceinline__ uint8_t e4m3_quant(float y, float s) { return (uint8_t)e4m3x2(__fdiv_rn(y, s), 0.f); }
+
+// 16 results of one lane, divided by the row scale, as one 16-byte vector of e4m3
+__device__ __forceinline__ uint4 e4m3_pack16(const float* f, float s) {
+  uint32_t w[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+    w[j] = e4m3x2(__fdiv_rn(f[4 * j], s), __fdiv_rn(f[4 * j + 1], s)) |
+           (e4m3x2(__fdiv_rn(f[4 * j + 2], s), __fdiv_rn(f[4 * j + 3], s)) << 16);
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
 
 
 // workspace layout of the row-split kernels (work counters, deferred segments, partials)

@@ -226,6 +226,48 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
       }
     }
   }
+
+  // final write of one row as e4m3 with its own scale (tsb200_spmm_fw_fp8_quant; T = float, one column tile). Called
+  // by all LPR lanes that hold the row (group 0 of a row-per-warp kernel, a row's own group in the group-per-row
+  // kernel): the row's amax is a shuffle over exactly those lanes, then every lane writes its 16 bytes per chunk.
+  __device__ __forceinline__ void store_row_q8(uint8_t* __restrict__ out_row, float* __restrict__ scale_out,
+                                               int64_t* __restrict__ arg_row, int64_t count, int64_t E,
+                                               const bool (&col_ok)[CH], int li, bool mean) {
+    static_assert(VEC == 16 && std::is_same<T, float>::value, "e4m3 result: fp8 operand, fp32 accumulation");
+    float amax = 0.f;
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) {
+      if (!col_ok[ch]) continue;
+#pragma unroll
+      for (int i = 0; i < VEC; i++) {
+        float a = acc[ch * VEC + i];
+        if (RED == R_SUM && mean) a = a / (float)(count > 0 ? count : 1);
+        if (ARG && count == 0) a = 0.f;
+        acc[ch * VEC + i] = a;
+        amax = amax_nan(amax, fabsf(a));
+      }
+    }
+    const unsigned gmask = LPR == 32 ? 0xffffffffu : (((1u << LPR) - 1u) << ((threadIdx.x & 31) & ~(LPR - 1)));
+#pragma unroll
+    for (int off = 1; off < LPR; off <<= 1) amax = amax_nan(amax, __shfl_xor_sync(gmask, amax, off));
+    const float s = e4m3_row_scale(amax);
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) {
+      if (!col_ok[ch]) continue;
+      const int koff = (ch * LPR + li) * VEC;
+      stg128_stream(out_row + koff, e4m3_pack16(&acc[ch * VEC], s));
+      if (ARG) {
+#pragma unroll
+        for (int i = 0; i < VEC; i += 2) {
+          longlong2 a2;
+          a2.x = (count > 0 && arg[ch * VEC + i] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i] : E;
+          a2.y = (count > 0 && arg[ch * VEC + i + 1] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i + 1] : E;
+          stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
+        }
+      }
+    }
+    if (li == 0) *scale_out = s;
+  }
 };
 
 // ---- packed 16-bit min/max engine --------------------------------------------------------------
@@ -420,6 +462,30 @@ template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, cons
   }
 }
 
+// column kk of a multi-segment row: its partials folded in segment order (min/max: the smallest e wins ties), the
+// mean's division applied. CG: read past L1 (partials written by other SMs during the same launch).
+template <int RED, bool CG>
+__device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow& L, int nseg, int64_t count,
+                                             int64_t kk, int64_t& ar) {
+  constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
+  const float* pv = (const float*)p.part_val;
+  float a = CG ? __ldcg(pv + L.first_slot * p.K + kk) : pv[L.first_slot * p.K + kk];
+  ar = 0;
+  if (ARG) ar = CG ? __ldcg(p.part_arg + L.first_slot * p.K + kk) : p.part_arg[L.first_slot * p.K + kk];
+  for (int sgi = 1; sgi < nseg; sgi++) {
+    const float v = CG ? __ldcg(pv + (L.first_slot + sgi) * p.K + kk) : pv[(L.first_slot + sgi) * p.K + kk];
+    if (RED == R_SUM) a += v;
+    else {
+      const int64_t va = CG ? __ldcg(p.part_arg + (L.first_slot + sgi) * p.K + kk)
+                            : p.part_arg[(L.first_slot + sgi) * p.K + kk];
+      const bool better = (RED == R_MIN) ? (v < a) : (v > a);
+      if (better || (v == a && va < ar)) { a = v; ar = va; }
+    }
+  }
+  if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
+  return a;
+}
+
 // combine the partials of one multi-segment row, in segment order, by ONE WARP (planned mode: the warp that finished
 // the row's last segment); the partials were written by other SMs -> read them past L1
 template <typename T, int RED>
@@ -447,7 +513,36 @@ __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const Long
   }
 }
 
-template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T>
+// the same for an e4m3 result (QO): a first pass over the partials finds the row's amax, the second writes y / scale
+template <int RED>
+__device__ __forceinline__ void combine_row_warp_q8(const SpmmParams& p, const LongRow& L, int lane, int kcols) {
+  constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
+  const int nseg = (int)(L.nseg_count >> 40);
+  const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+  float amax = 0.f;
+  for (int k = lane; k < kcols; k += 32) {
+    const int64_t kk = p.k0 + k;
+    if (kk >= p.K) break;
+    int64_t ar;
+    amax = amax_nan(amax, fabsf(combine_col<RED, true>(p, L, nseg, count, kk, ar)));
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+  const float s = e4m3_row_scale(amax);
+  if (lane == 0) p.out_scale[L.row_b] = s;
+  for (int k = lane; k < kcols; k += 32) {
+    const int64_t kk = p.k0 + k;
+    if (kk >= p.K) break;
+    int64_t ar;
+    const float a = combine_col<RED, true>(p, L, nseg, count, kk, ar);
+    ((uint8_t*)p.out)[L.row_b * p.K + kk] = e4m3_quant(a, s);
+    if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
+  }
+}
+
+// QO: e4m3 result with per-row scales (RowEngine::store_row_q8) instead of T
+template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
+          bool QO = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_vec_kernel(const SpmmParams p) {
   using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
@@ -561,8 +656,14 @@ spmm_vec_kernel(const SpmmParams p) {
       set_scale(eng, p);
       eng.accumulate(ring, s, e, matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
-      if (g == 0) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
-                                ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+      if constexpr (QO) {
+        if (g == 0)
+          eng.store_row_q8((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
+                           argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0);
+      } else {
+        if (g == 0) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
+                                  ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+      }
     }
     item = __shfl_sync(0xffffffffu, next_item, 0);
   }
@@ -589,9 +690,15 @@ spmm_vec_kernel(const SpmmParams p) {
       eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
       if (S.slot < 0) {
-        if (g == 0)
-          eng.store_row((T*)p.out + row * p.K + p.k0, p.arg_out ? p.arg_out + row * p.K + p.k0 : nullptr,
-                        S.end - S.start, p.E, col_ok, li, p.mean != 0);
+        if constexpr (QO) {
+          if (g == 0)
+            eng.store_row_q8((uint8_t*)p.out + row * p.K, p.out_scale + row, p.arg_out ? p.arg_out + row * p.K : nullptr,
+                             S.end - S.start, p.E, col_ok, li, p.mean != 0);
+        } else {
+          if (g == 0)
+            eng.store_row((T*)p.out + row * p.K + p.k0, p.arg_out ? p.arg_out + row * p.K + p.k0 : nullptr,
+                          S.end - S.start, p.E, col_ok, li, p.mean != 0);
+        }
       } else {
         if (g == 0) {
           float* pv = (float*)p.part_val + S.slot * p.K + p.k0;
@@ -616,7 +723,8 @@ spmm_vec_kernel(const SpmmParams p) {
         const LongRow L = p.longs[lr];
         if ((int)finished == (int)(L.nseg_count >> 40) - 1) {
           __threadfence();
-          combine_row_warp<T, RED>(p, L, lane, kcols);
+          if constexpr (QO) combine_row_warp_q8<RED>(p, L, lane, kcols);
+          else combine_row_warp<T, RED>(p, L, lane, kcols);
         }
       }
       __syncwarp();
@@ -639,7 +747,8 @@ template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __
   return __ldg(reinterpret_cast<const unsigned short*>(p));
 }
 
-template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T>
+template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
+          bool QO = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_gpr_kernel(const SpmmParams p) {
   using V = Vec<T>;
@@ -788,15 +897,21 @@ spmm_gpr_kernel(const SpmmParams p) {
           else eng.minmax_step(eng.acc, eng.arg, V::vfloat(v[u]), d[u], jbase + s + j0 + u);
         }
       }
-      if (mine) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
-                              p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+      if constexpr (QO) {  // `mine` is the same for the LPR lanes of a group, so the group's amax shuffle is complete
+        if (mine)
+          eng.store_row_q8((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
+                           argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li, p.mean != 0);
+      } else {
+        if (mine) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
+                                p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+      }
     }
     item = __shfl_sync(0xffffffffu, next_item, 0);
   }
 }
 
 // one warp per queued segment
-template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T>
+template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T, bool QO = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_seg_kernel(const SpmmParams p) {
   using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
@@ -842,10 +957,14 @@ spmm_seg_kernel(const SpmmParams p) {
     eng.reduce_groups();
     if (g == 0) {
       if (S.slot < 0) {
-        eng.store_row((T*)p.out + (b * p.M + row) * p.K + p.k0,
-                      p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
-                      S.end - S.start, p.E, col_ok, li, p.mean != 0,
-                      ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0);
+        if constexpr (QO)
+          eng.store_row_q8((uint8_t*)p.out + row * p.K, p.out_scale + row, p.arg_out ? p.arg_out + row * p.K : nullptr,
+                           S.end - S.start, p.E, col_ok, li, p.mean != 0);
+        else
+          eng.store_row((T*)p.out + (b * p.M + row) * p.K + p.k0,
+                        p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
+                        S.end - S.start, p.E, col_ok, li, p.mean != 0,
+                        ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0);
       } else {
         float* pv = (float*)p.part_val + S.slot * p.K + p.k0;
         int64_t* pa = Eng::ARG ? p.part_arg + S.slot * p.K + p.k0 : nullptr;
@@ -895,6 +1014,45 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
         if (p.acc_mode != 3) { *pr = a; continue; }
       }
       ((T*)p.out)[L.row_b * p.K + kk] = Traits<T>::from_acc(a);
+      if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
+    }
+  }
+}
+
+// the same for an e4m3 result (QO): per row, a first pass over the partials and a block reduction find the row's amax,
+// the second pass writes y / scale
+constexpr int kCombineThreads = 128;
+template <int RED>
+__global__ void __launch_bounds__(kCombineThreads) spmm_combine_q8_kernel(const SpmmParams p, int kcols) {
+  constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
+  __shared__ float s_amax[kCombineThreads / 32];
+  const int64_t nlong = p.plan_mask ? p.n_long : min((int64_t)p.counters[2], p.long_cap);
+  for (int64_t li = blockIdx.x; li < nlong; li += gridDim.x) {
+    const LongRow L = p.longs[li];
+    const int nseg = (int)(L.nseg_count >> 40);
+    const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+    float amax = 0.f;
+    for (int k = threadIdx.x; k < kcols; k += kCombineThreads) {
+      const int64_t kk = p.k0 + k;
+      if (kk >= p.K) break;
+      int64_t ar;
+      amax = amax_nan(amax, fabsf(combine_col<RED, false>(p, L, nseg, count, kk, ar)));
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+    if ((threadIdx.x & 31) == 0) s_amax[threadIdx.x >> 5] = amax;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < kCombineThreads / 32; w++) amax = amax_nan(amax, s_amax[w]);
+    __syncthreads();  // s_amax is rewritten for the next row
+    const float s = e4m3_row_scale(amax);
+    if (threadIdx.x == 0) p.out_scale[L.row_b] = s;
+    for (int k = threadIdx.x; k < kcols; k += kCombineThreads) {
+      const int64_t kk = p.k0 + k;
+      if (kk >= p.K) break;
+      int64_t ar;
+      const float a = combine_col<RED, false>(p, L, nseg, count, kk, ar);
+      ((uint8_t*)p.out)[L.row_b * p.K + kk] = e4m3_quant(a, s);
       if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
     }
   }
@@ -968,16 +1126,22 @@ static bool vec_eligible(int dtype, int64_t K, int64_t E, int64_t N, const void*
   return true;
 }
 
+template <typename T, int RED, bool QO>
+static void launch_combine(const SpmmParams& p, int kcols, cudaStream_t st) {
+  if constexpr (QO) spmm_combine_q8_kernel<RED><<<num_sms() * 2, kCombineThreads, 0, st>>>(p, kcols);
+  else spmm_combine_kernel<T, RED><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
+}
+
 template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false,
-          typename X = T>
+          typename X = T, bool QO = false>
 static int launch_vec(SpmmParams p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(X);
   constexpr int kcols = LPR * CH * VEC;
   void (*kmain)(const SpmmParams);
-  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X>;
-  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X>;
+  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X, QO>;
+  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X, QO>;
   constexpr int USEG = (U > LPR) ? LPR : U;  // the row engine needs U * (32 / LPR) <= 32
-  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X>;
+  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   // small matrices: shrink the work item so that every resident warp gets rows
@@ -1003,7 +1167,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
         kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
         TSB_LAUNCH_CHECK();
         if (p.n_long > 0) {
-          spmm_combine_kernel<T, RED><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
+          launch_combine<T, RED, QO>(p, kcols, st);
           TSB_LAUNCH_CHECK();
         }
       }
@@ -1015,7 +1179,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
       TSB_LAUNCH_CHECK();
       kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
       TSB_LAUNCH_CHECK();
-      spmm_combine_kernel<T, RED><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
+      launch_combine<T, RED, QO>(p, kcols, st);
       TSB_LAUNCH_CHECK();
     }
   }
@@ -1025,7 +1189,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
 // (LPR, CH) follow from the width of a dense row; (U, MINB) = gathers in flight per lane and CTAs
 // per SM: the kernel is HBM-latency bound, so resident warps x gathers-in-flight wins (40 warps/SM x 4 x 16 B
 // per lane; the register budget of MINB = 5 is the same 64K registers per SM on sm_90).
-template <typename T, int RED, bool ACC = false, bool PLAN = false, typename X = T>
+template <typename T, int RED, bool ACC = false, bool PLAN = false, typename X = T, bool QO = false>
 static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   // fp8 operand: a vector is 16 columns, so a lane keeps twice the accumulators (and arg slots) of a 16-bit operand
   // and needs more registers per thread: its own (U, CTAs/SM) per shape (ptxas report and times in DESIGN §3.1)
@@ -1035,28 +1199,31 @@ static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row
   // narrow rows: group-per-row kernel (all reductions)
   constexpr int GB = Q8 ? (MM ? 2 : 3) : 5;
-  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X>(p, st);
-  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X>(p, st);
-  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X>(p, st);
-  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, GB, true, PLAN, X>(p, st);
+  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X, QO>(p, st);
+  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X, QO>(p, st);
+  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X, QO>(p, st);
+  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, GB, true, PLAN, X, QO>(p, st);
   // 256-byte rows (F = 128 bf16): at MINB = 5 the 48-register budget spills (120 B of stack in the planned kernel);
   // 3 CTAs/SM with 6 gathers in flight per lane is 8 % faster at C2 on the H100 (sweep in DESIGN §3.1)
+  // e4m3 result (QO): the quantising epilogue (row amax, IEEE divisions) spills the sum kernels of 256-, 512- and
+  // 2048-byte rows at the CTAs/SM of the fp32 result; those take one CTA/SM less (ptxas table in DESIGN §3.1)
   if (vecs <= 16)
-    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && MM ? 2 : 3, false, PLAN, X>(p, st);
-  if (vecs <= 32) return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (MM ? 2 : 3) : 5, false, PLAN, X>(p, st);
-  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X>(p, st);
+    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && (MM || QO) ? 2 : 3, false, PLAN, X, QO>(p, st);
+  if (vecs <= 32)
+    return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (MM || QO ? 2 : 3) : 5, false, PLAN, X, QO>(p, st);
+  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X, QO>(p, st);
   // column-tiled beyond 128 vectors
-  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (MM ? 1 : 2) : 3, false, PLAN, X>(p, st);
+  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (MM || QO ? 1 : 2) : 3, false, PLAN, X, QO>(p, st);
 }
 
-template <typename T, bool PLAN = false, typename X = T>
+template <typename T, bool PLAN = false, typename X = T, bool QO = false>
 static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
   p.mean = (reduce == TSB200_MEAN);
   switch (reduce) {
     case TSB200_SUM:
-    case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN, X>(p, st);
-    case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN, X>(p, st);
-    case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN, X>(p, st);
+    case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN, X, QO>(p, st);
+    case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN, X, QO>(p, st);
+    case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN, X, QO>(p, st);
   }
   return TSB200_ERR_INVALID_ARG;
 }
@@ -1348,23 +1515,50 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
 
 // ---- SpMM over an fp8 (e4m3) dense operand with per-tensor or per-row scales ----------------------------------------
 // The same kernels, instantiated with X = __nv_fp8_e4m3: value / output type T = out_dtype, a dense row is K bytes.
-extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
-                                  const float* scale, int64_t scale_stride, void* out, int64_t* arg_out, int64_t M,
-                                  int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
-                                  size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
-                                  size_t workspace_bytes, void* stream) {
+// out_scale != NULL: e4m3 result with per-row scales (tsb200_spmm_fw_fp8_quant): T = float, `out` is e4m3 [M, K].
+namespace tsb {
+__global__ void fill_f32_kernel(float* __restrict__ p, int64_t n, float v) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
+}
+
+template <bool PLAN, bool QO>
+static int dispatch_fp8_out(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
+  if constexpr (QO) return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, true>(p, reduce, st);
+  switch (out_dtype) {
+    case TSB200_F32: return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3>(p, reduce, st);
+    case TSB200_F16: return dispatch_red_vec<__half, PLAN, __nv_fp8_e4m3>(p, reduce, st);
+    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, PLAN, __nv_fp8_e4m3>(p, reduce, st);
+  }
+  return TSB200_ERR_UNSUPPORTED;
+}
+
+template <bool QO>
+static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                            const float* scale, int64_t scale_stride, void* out, float* out_scale, int64_t* arg_out,
+                            int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
+                            size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                            size_t workspace_bytes, void* stream) {
   if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
   if (reduce < TSB200_SUM || reduce > TSB200_MAX) return TSB200_ERR_INVALID_ARG;
   if (scale_stride != 0 && scale_stride != 1) return TSB200_ERR_INVALID_ARG;
   if (out_dtype != TSB200_F32 && out_dtype != TSB200_F16 && out_dtype != TSB200_BF16) return TSB200_ERR_UNSUPPORTED;
   if (K % 16 != 0) return TSB200_ERR_UNSUPPORTED;
+  // e4m3 result: a row's amax is taken inside one column tile of the kernels (at most 2048 fp8 columns)
+  if (QO && K > 2048) return TSB200_ERR_UNSUPPORTED;
   const bool arg = (reduce == TSB200_MIN || reduce == TSB200_MAX);
-  if (M * K == 0) return 0;
-  if (!rowptr || !out || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
+  if (M == 0 || (!QO && K == 0)) return 0;
+  if (!rowptr || !out || (QO && !out_scale) || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
+  if (QO && ((uintptr_t)out_scale & 3)) return TSB200_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
-  if (E == 0) {  // every row is empty: 0, and arg_out = E = 0
-    TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(M * K) * dtype_size(out_dtype), st));
-    if (arg) TSB_CUDA_TRY(cudaMemsetAsync(arg_out, 0, (size_t)(M * K) * sizeof(int64_t), st));
+  if (E == 0 || K == 0) {  // every row is empty: 0, arg_out = E = 0, and a scale of 1 (an amax of 0)
+    if (K > 0) {
+      TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(M * K) * (QO ? 1 : dtype_size(out_dtype)), st));
+      if (arg) TSB_CUDA_TRY(cudaMemsetAsync(arg_out, 0, (size_t)(M * K) * sizeof(int64_t), st));
+    }
+    if (QO) {
+      fill_f32_kernel<<<(int)min((M + 255) / 256, (int64_t)num_sms() * 8), 256, 0, st>>>(out_scale, M, 1.f);
+      TSB_LAUNCH_CHECK();
+    }
     return 0;
   }
   if (!col || !mat || !scale) return TSB200_ERR_INVALID_ARG;
@@ -1379,6 +1573,7 @@ extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, con
   p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
   p.partial = nullptr; p.acc_mode = 0;
   p.scale = scale; p.scale_stride = (uint32_t)scale_stride;
+  p.out_scale = out_scale;
   if (plan) {  // planned: the layout of tsb200_spmm_fw_planned
     const PlanLayout PL = plan_layout(M, E);
     if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
@@ -1396,12 +1591,7 @@ extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, con
     p.part_val = ws + W.part_val;
     p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
     p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
-    switch (out_dtype) {
-      case TSB200_F32: return dispatch_red_vec<float, true, __nv_fp8_e4m3>(p, reduce, st);
-      case TSB200_F16: return dispatch_red_vec<__half, true, __nv_fp8_e4m3>(p, reduce, st);
-      case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, true, __nv_fp8_e4m3>(p, reduce, st);
-    }
-    return TSB200_ERR_UNSUPPORTED;
+    return dispatch_fp8_out<true, QO>(p, out_dtype, reduce, st);
   }
   // unplanned: the layout of tsb200_spmm_fw (tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce))
   const WsLayout L = ws_layout(1, K, E, arg);
@@ -1413,10 +1603,26 @@ extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, con
   p.part_val = ws + L.part_val;
   p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
   p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
-  switch (out_dtype) {
-    case TSB200_F32: return dispatch_red_vec<float, false, __nv_fp8_e4m3>(p, reduce, st);
-    case TSB200_F16: return dispatch_red_vec<__half, false, __nv_fp8_e4m3>(p, reduce, st);
-    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, false, __nv_fp8_e4m3>(p, reduce, st);
-  }
-  return TSB200_ERR_UNSUPPORTED;
+  return dispatch_fp8_out<false, QO>(p, out_dtype, reduce, st);
+}
+}  // namespace tsb
+
+extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                  const float* scale, int64_t scale_stride, void* out, int64_t* arg_out, int64_t M,
+                                  int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
+                                  size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return spmm_fw_fp8_impl<false>(rowptr, col, value, mat, scale, scale_stride, out, nullptr, arg_out, M, N, K, E,
+                                 out_dtype, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes,
+                                 stream);
+}
+
+extern "C" int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                        const float* scale, int64_t scale_stride, void* out8, float* out_scale,
+                                        int64_t* arg_out, int64_t M, int64_t N, int64_t K, int64_t E, int reduce,
+                                        const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                                        int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream) {
+  return spmm_fw_fp8_impl<true>(rowptr, col, value, mat, scale, scale_stride, out8, out_scale, arg_out, M, N, K, E,
+                                TSB200_F32, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace,
+                                workspace_bytes, stream);
 }

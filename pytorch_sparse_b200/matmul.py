@@ -96,6 +96,23 @@ def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
     return torch.ops.tsb200.spmm_fp8(rowptr, col, value, x8, scale, reduce, out_dtype)[0]
 
 
+def spmm_fp8_quant(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum") -> Tuple[Tensor, Tensor]:
+    """One FP8 propagation hop: `src @ (x8 * scale)` as `spmm_fp8(..., torch.float32)` computes it, returned as
+    `(y8, y_scale)` = `quantize_fp8(y, per_row=True)` of that float32 result, bit for bit, without materialising y:
+    the kernels quantise each row as they store it. The pair is the `x8` / `scale` of the next hop, so repeated
+    propagation (SIGN, APPNP, label propagation) stays in e4m3. K <= 2048 columns; entry values are cast to float32.
+    Forward only: a `value` or `scale` that requires grad is refused while grad mode is on."""
+    rowptr, col, value = src.csr()
+    if value is not None:
+        value = value.to(torch.float32)
+    if reduce == "add":
+        reduce = "sum"
+    if reduce != "sum" and reduce != "mean" and reduce != "min" and reduce != "max":
+        raise ValueError("unknown reduce '" + reduce + "'")
+    y8, y_scale, _ = torch.ops.tsb200.spmm_fp8_quant(rowptr, col, value, x8, scale, reduce)
+    return y8, y_scale
+
+
 def quantize_fp8(x: Tensor, per_row: bool = True) -> Tuple[Tensor, Tensor]:
     """A 2-D floating `x` [N, K] as `(x8, scale)` for `spmm_fp8`: scale = amax|x| / 448 (e4m3's largest finite value)
     per row ([N]) or over the whole tensor ([]), 1 where that amax is 0, and x8 = e4m3(x / scale), rounded to
@@ -165,6 +182,7 @@ def matmul(src, other, reduce="sum"):  # noqa: F811
 SparseTensor.spmm = lambda self, other, reduce="sum": spmm(self, other, reduce)
 SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bfloat16: spmm_fp8(
     self, x8, scale, reduce, out_dtype)
+SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum": spmm_fp8_quant(self, x8, scale, reduce)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)
 SparseTensor.__matmul__ = lambda self, other: matmul(self, other, "sum")

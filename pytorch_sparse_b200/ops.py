@@ -212,6 +212,59 @@ def spmm_fw(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor,
 _FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
 
 
+def _fp8_args(what: str, rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
+              out_dtype: Optional[torch.dtype]):
+    """The checks shared by spmm_fw_fp8 (out_dtype given) and spmm_fw_fp8_quant (None: float32 values);
+    returns (rowptr, col, value, scale, scale_stride)."""
+    _check_cuda(rowptr, "rowptr")
+    _check_cuda(col, "col")
+    if value is not None:
+        _check_cuda(value, "optional_value.value()")
+    _check_cuda(x8, "x8")
+    _check_cuda(scale, "scale")
+    if torch.is_grad_enabled() and (scale.requires_grad or (value is not None and value.requires_grad)):
+        raise RuntimeError(f"{what} is forward only: value and scale must not require grad "
+                           "(call it under torch.no_grad() or detach them)")
+    if x8.dtype != torch.float8_e4m3fn:
+        raise RuntimeError(f"{what}: x8 must be torch.float8_e4m3fn, got {x8.dtype}")
+    if x8.dim() != 2:
+        raise RuntimeError(f"{what}: x8 must be 2-D [N, K], got {x8.dim()}-D")
+    N, K = x8.shape
+    if K % 16 != 0:
+        raise RuntimeError(f"{what}: the number of columns K = {K} must be a multiple of 16")
+    if not x8.is_contiguous() or x8.data_ptr() % 16 != 0:
+        raise RuntimeError(f"{what}: x8 must be contiguous and 16-byte aligned")
+    if out_dtype is not None and out_dtype not in _FP8_OUT:
+        raise RuntimeError(f"{what}: out_dtype must be torch.bfloat16, torch.float16 or torch.float32, got {out_dtype}")
+    value_dtype = torch.float32 if out_dtype is None else out_dtype
+    if scale.dtype != torch.float32:
+        raise RuntimeError(f"{what}: scale must be float32, got {scale.dtype}")
+    if scale.dim() == 0:
+        stride = 0
+    elif scale.dim() == 1 and scale.size(0) == N:
+        stride = 1
+    else:
+        raise RuntimeError(f"{what}: scale must have shape [] or [N] = [{N}], got {list(scale.shape)}")
+    scale = scale.contiguous()
+    _check_input(rowptr.dim() == 1)
+    _check_input(col.dim() == 1)
+    if value is not None:
+        _check_input(value.dim() == 1)
+        _check_input(value.size(0) == col.size(0))
+        if value.dtype != value_dtype:
+            raise RuntimeError(f"expected value of dtype {value_dtype} but got {value.dtype}")
+        value = value.contiguous()
+    return _i64(rowptr, "rowptr"), _i64(col, "col"), value, scale, stride
+
+
+def _fp8_plan(plan: Optional[SpmmPlan], rowptr: Tensor, M: int, E: int) -> Optional[SpmmPlan]:
+    if plan is None:
+        plan = _auto_plan(rowptr, E)
+    if plan is not None and (plan.M != M or plan.E != E):
+        plan = None
+    return plan
+
+
 def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
                 reduce: str = "sum", out_dtype: torch.dtype = torch.bfloat16,
                 plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor]]:
@@ -221,46 +274,9 @@ def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor
     `out_dtype` (bf16, f16 or f32), as `spmm_fw`'s value has the dense dtype. Entry e weighs fl32(value[e] * scale[c]);
     sums accumulate weight * x8 in fp32 and round once, min/max compare the product rounded to `out_dtype`. Forward
     only. Planned like `spmm_fw` (the same per-rowptr plan cache)."""
-    _check_cuda(rowptr, "rowptr")
-    _check_cuda(col, "col")
-    if value is not None:
-        _check_cuda(value, "optional_value.value()")
-    _check_cuda(x8, "x8")
-    _check_cuda(scale, "scale")
-    if torch.is_grad_enabled() and (scale.requires_grad or (value is not None and value.requires_grad)):
-        raise RuntimeError("spmm_fp8 is forward only: value and scale must not require grad "
-                           "(call it under torch.no_grad() or detach them)")
-    if x8.dtype != torch.float8_e4m3fn:
-        raise RuntimeError(f"spmm_fp8: x8 must be torch.float8_e4m3fn, got {x8.dtype}")
-    if x8.dim() != 2:
-        raise RuntimeError(f"spmm_fp8: x8 must be 2-D [N, K], got {x8.dim()}-D")
-    N, K = x8.shape
-    if K % 16 != 0:
-        raise RuntimeError(f"spmm_fp8: the number of columns K = {K} must be a multiple of 16")
-    if not x8.is_contiguous() or x8.data_ptr() % 16 != 0:
-        raise RuntimeError("spmm_fp8: x8 must be contiguous and 16-byte aligned")
-    if out_dtype not in _FP8_OUT:
-        raise RuntimeError(f"spmm_fp8: out_dtype must be torch.bfloat16, torch.float16 or torch.float32, got {out_dtype}")
-    if scale.dtype != torch.float32:
-        raise RuntimeError(f"spmm_fp8: scale must be float32, got {scale.dtype}")
-    if scale.dim() == 0:
-        stride = 0
-    elif scale.dim() == 1 and scale.size(0) == N:
-        stride = 1
-    else:
-        raise RuntimeError(f"spmm_fp8: scale must have shape [] or [N] = [{N}], got {list(scale.shape)}")
-    scale = scale.contiguous()
-    _check_input(rowptr.dim() == 1)
-    _check_input(col.dim() == 1)
-    if value is not None:
-        _check_input(value.dim() == 1)
-        _check_input(value.size(0) == col.size(0))
-        if value.dtype != out_dtype:
-            raise RuntimeError(f"expected value of dtype {out_dtype} but got {value.dtype}")
-        value = value.contiguous()
+    rowptr, col, value, scale, stride = _fp8_args("spmm_fp8", rowptr, col, value, x8, scale, out_dtype)
     red = _reduce_code(reduce)
-    rowptr = _i64(rowptr, "rowptr")
-    col = _i64(col, "col")
+    N, K = x8.shape
     M, E = rowptr.numel() - 1, col.numel()
     dev = x8.device
     out = torch.empty(M, K, dtype=out_dtype, device=dev)
@@ -273,10 +289,7 @@ def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor
             arg_out.fill_(0)
         return out, arg_out
     with _on_device(dev):
-        if plan is None:
-            plan = _auto_plan(rowptr, E)
-        if plan is not None and (plan.M != M or plan.E != E):
-            plan = None
+        plan = _fp8_plan(plan, rowptr, M, E)
         if plan is not None:
             nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
             pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
@@ -288,6 +301,50 @@ def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor
                                      M, N, K, E, _FP8_OUT[out_dtype], red, pl, pl_bytes, *counts, _p(ws), nws,
                                      _stream(dev)), "tsb200_spmm_fw_fp8")
     return out, arg_out
+
+
+FP8_QUANT_MAX_K = 2048
+
+
+def spmm_fw_fp8_quant(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
+                      reduce: str = "sum",
+                      plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Tensor, Optional[Tensor]]:
+    """`spmm_fw_fp8_quant(rowptr, col, optional_value, x8, scale, reduce) -> (y8, y_scale, arg_out?)`
+    (tsb200_spmm_fw_fp8_quant): `spmm_fw_fp8` with a float32 result y, written as e4m3 with one scale per row by the
+    kernel itself: y_scale[m] = amax|y[m]| / 448 (1 when that is not > 0, NaN rows included) and y8 = e4m3(y / y_scale),
+    bit for bit `quantize_fp8(y, per_row=True)` on the CPU. `value` is float32. (y8, y_scale) are the `x8` and `scale`
+    of the next hop. K <= 2048. Forward only; planned like `spmm_fw` (the same per-rowptr plan cache)."""
+    rowptr, col, value, scale, stride = _fp8_args("spmm_fp8_quant", rowptr, col, value, x8, scale, None)
+    N, K = x8.shape
+    if K > FP8_QUANT_MAX_K:
+        raise RuntimeError(f"spmm_fp8_quant: the number of columns K = {K} must be at most {FP8_QUANT_MAX_K}")
+    red = _reduce_code(reduce)
+    M, E = rowptr.numel() - 1, col.numel()
+    dev = x8.device
+    y8 = torch.empty(M, K, dtype=torch.float8_e4m3fn, device=dev)
+    y_scale = torch.empty(M, dtype=torch.float32, device=dev)
+    arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
+    if M == 0:
+        return y8, y_scale, arg_out
+    if E == 0 or K == 0:
+        y8.zero_()
+        y_scale.fill_(1.0)
+        if arg_out is not None:
+            arg_out.fill_(0)
+        return y8, y_scale, arg_out
+    with _on_device(dev):
+        plan = _fp8_plan(plan, rowptr, M, E)
+        if plan is not None:
+            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
+            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
+        else:
+            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, _FP8_OUT[torch.float32], red)
+            pl, pl_bytes, counts = None, 0, (0, 0, 0)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_fw_fp8_quant(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(y8),
+                                           _p(y_scale), _p(arg_out), M, N, K, E, red, pl, pl_bytes, *counts, _p(ws),
+                                           nws, _stream(dev)), "tsb200_spmm_fw_fp8_quant")
+    return y8, y_scale, arg_out
 
 
 def spmm_fw_acc(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, partial: Tensor,

@@ -2,7 +2,7 @@
 (csrc/spmm.cpp:305-348, csrc/convert.cpp:46-48):
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
-    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8}   (this package's own additions)
+    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -45,6 +45,8 @@ _EXTRA_SCHEMAS = {
               "int M, int K, int N, bool want_value) -> (Tensor, Tensor, Tensor, Tensor?)",
     "spmm_fp8": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
                 "ScalarType out_dtype) -> (Tensor, Tensor?)",
+    "spmm_fp8_quant": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce) "
+                      "-> (Tensor, Tensor, Tensor?)",
 }
 
 
@@ -60,6 +62,8 @@ _EXTRA_IMPLS = {
     "spspmm": ops.spspmm,
     "spmm_fp8": lambda rowptr, col, value, x8, scale, reduce, out_dtype: ops.spmm_fw_fp8(rowptr, col, value, x8, scale,
                                                                                          reduce, out_dtype),
+    "spmm_fp8_quant": lambda rowptr, col, value, x8, scale, reduce: ops.spmm_fw_fp8_quant(rowptr, col, value, x8,
+                                                                                          scale, reduce),
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -158,6 +158,32 @@ TSB200_API int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* co
                                         int64_t n_long, int64_t n_slot, void* workspace, size_t workspace_bytes,
                                         void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * FP8 SpMM with a per-row e4m3 residual added in the store epilogue, for propagation with a fixed residual term
+ * (APPNP: X_{h+1} = (1-a) A X_h + a H; label propagation: Y_{h+1} = a A Y_h + (1-a) Y_0) without leaving e4m3
+ * (no counterpart in the reference).  B = 1, SUM / MEAN only.
+ *   Let y[m,k] be the F32 value tsb200_spmm_fw_fp8 writes with the same arguments and out_dtype = TSB200_F32, on the
+ *   same path (planned or unplanned): after the mean's division, +0 on an empty row. With
+ *     rho[m,k] = fl32(res_scale[m * res_scale_stride] * e4m3(res8[m,k]))    (res_scale_stride 0 or 1)
+ *     z[m,k]   = fl32(y[m,k] + rho[m,k])                                     (one IEEE add, no FMA contraction)
+ *   out_scale == NULL: out out_dtype[M, K] = round_out(z) (round to nearest even), value out_dtype[E] or NULL.
+ *   out_scale != NULL: the e4m3 result of tsb200_spmm_fw_fp8_quant with z in place of y (bit for bit torch's
+ *   quantize_fp8(z, per_row=True) on the CPU); out e4m3[M, K], value f32[E] or NULL, out_dtype must be TSB200_F32,
+ *   K <= 2048. NaN and +-inf propagate through z as IEEE says (a -0 residual on an empty row gives +0).
+ *   res8 e4m3[M, K] contiguous, 16-byte aligned; res_scale f32, 4-byte aligned. The caller folds propagation weights
+ *   into the entry values and res_scale. E == 0: z = fl32(+0 + rho).
+ *   Plan and workspace sizing as tsb200_spmm_fw_fp8 (with out_dtype = TSB200_F32 for an e4m3 result).
+ *   res8 == NULL: exactly tsb200_spmm_fw_fp8 (out_scale == NULL) or tsb200_spmm_fw_fp8_quant, MIN / MAX included.
+ *   TSB200_ERR_UNSUPPORTED for MIN / MAX with a residual, a misaligned res8 (16 B) or res_scale (4 B), and as
+ *   tsb200_spmm_fw_fp8 / _quant otherwise.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                      const float* scale, int64_t scale_stride, const void* res8,
+                                      const float* res_scale, int64_t res_scale_stride, void* out, float* out_scale,
+                                      int64_t* arg_out, int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype,
+                                      int reduce, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                                      int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream);
+
 /* One COLUMN BLOCK of a SUM SpMM (multi-GPU pipelining: the dense operand arrives block by block over NVLink and
  * block p of A's columns is multiplied as soon as block p of `mat` has landed; no counterpart in the reference, which
  * has no collectives — the partitioner semantics are torch_sparse/narrow.py:15-42). (rowptr, col, value) hold only the

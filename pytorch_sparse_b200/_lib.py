@@ -36,6 +36,10 @@ SIGNATURES = {
     "tsb200_spmm_fw_fp8_quant": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
                                          c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t,
                                          c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_fw_fp8_res": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                       c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                       c_int, c_int, c_void_p, c_size_t, c_int64, c_int64, c_int64, c_void_p,
+                                       c_size_t, c_void_p]),
     "tsb200_spmm_fw_acc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                    c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
     "tsb200_spmm_value_bw_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int]),

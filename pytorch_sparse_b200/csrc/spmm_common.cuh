@@ -62,6 +62,11 @@ struct SpmmParams {
   uint32_t scale_stride;
   // e4m3 result (tsb200_spmm_fw_fp8_quant): `out` is e4m3 [M, K], out_scale[m] = amax_k |y[m,k]| / 448 (1 if not > 0)
   float* out_scale;
+  // residual (tsb200_spmm_fw_fp8_res, RES kernels): row m of the result is y[m] + fl32(res_scale[m * res_stride] *
+  // res8[m]), res8 e4m3 [M, K], added after the mean's division and before the e4m3 quantisation
+  const uint8_t* res8;
+  const float* res_scale;
+  uint32_t res_stride;
 };
 
 // ---- per-warp streaming index ring ------------------------------------------------------------
@@ -279,6 +284,31 @@ __device__ __forceinline__ uint4 e4m3_pack16(const float* f, float s) {
     w[j] = e4m3x2(__fdiv_rn(f[4 * j], s), __fdiv_rn(f[4 * j + 1], s)) |
            (e4m3x2(__fdiv_rn(f[4 * j + 2], s), __fdiv_rn(f[4 * j + 3], s)) << 16);
   return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// ---- e4m3 residual (tsb200_spmm_fw_fp8_res) -------------------------------------------------------------------------
+// z = fl32(y + fl32(rs * r)): one IEEE product and one IEEE add, never contracted to an FMA. The residual is read once,
+// so it is loaded with the streaming (evict-first) hint.
+__device__ __forceinline__ float e4m3_to_f32(uint8_t b) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)b));
+  return __half2float(__ushort_as_half((unsigned short)(r & 0xffffu)));
+}
+__device__ __forceinline__ float res_add(float y, float rs, uint8_t r) {
+  return __fadd_rn(y, __fmul_rn(rs, e4m3_to_f32(r)));
+}
+// 16 consecutive results of one lane plus their 16 residual columns (one 16-byte load)
+__device__ __forceinline__ void res_add16(float* f, const uint8_t* r, float rs) {
+  float q[16];
+  Vec<__nv_fp8_e4m3>::unpack(__ldcs(reinterpret_cast<const uint4*>(r)), q);
+#pragma unroll
+  for (int i = 0; i < 16; i++) f[i] = __fadd_rn(f[i], __fmul_rn(rs, q[i]));
+}
+__device__ __forceinline__ const uint8_t* res_row(const SpmmParams& p, int64_t row) {
+  return p.res8 + row * p.K + p.k0;
+}
+__device__ __forceinline__ float res_scale(const SpmmParams& p, int64_t row) {
+  return __ldg(p.res_scale + row * p.res_stride);
 }
 
 

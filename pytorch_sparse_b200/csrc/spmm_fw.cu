@@ -182,10 +182,14 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
     }
   }
 
-  // final write of one row (group 0 lanes). count = row degree.
+  // final write of one row (group 0 lanes). count = row degree. RES: res_row is the row's residual at this launch's
+  // first column and rs its scale; the lane adds its 16 residual columns per chunk after the mean's division.
+  template <bool RES = false>
   __device__ __forceinline__ void store_row(T* __restrict__ out_row, int64_t* __restrict__ arg_row,
                                             int64_t count, int64_t E, const bool (&col_ok)[CH], int li,
-                                            bool mean, float* __restrict__ part_row = nullptr, int acc_mode = 0) {
+                                            bool mean, float* __restrict__ part_row = nullptr, int acc_mode = 0,
+                                            const uint8_t* __restrict__ res_row = nullptr, float rs = 0.f) {
+    static_assert(!RES || (Q8 && RED == R_SUM), "residual: fp8 operand, sum / mean");
 #pragma unroll
     for (int ch = 0; ch < CH; ch++) {
       if (!col_ok[ch]) continue;
@@ -198,6 +202,7 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
         f[i] = a;
       }
       const int koff = (ch * LPR + li) * VEC;
+      if constexpr (RES) res_add16(f, res_row + koff, rs);
       if (RED == R_SUM && acc_mode) {  // column-block pipelining: fp32 partial shared by the launches of one product
         float4* pr = reinterpret_cast<float4*>(part_row + koff);
         if (acc_mode != 1) {
@@ -230,10 +235,14 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
   // final write of one row as e4m3 with its own scale (tsb200_spmm_fw_fp8_quant; T = float, one column tile). Called
   // by all LPR lanes that hold the row (group 0 of a row-per-warp kernel, a row's own group in the group-per-row
   // kernel): the row's amax is a shuffle over exactly those lanes, then every lane writes its 16 bytes per chunk.
+  // RES: the residual is added (as in store_row) before the row amax.
+  template <bool RES = false>
   __device__ __forceinline__ void store_row_q8(uint8_t* __restrict__ out_row, float* __restrict__ scale_out,
                                                int64_t* __restrict__ arg_row, int64_t count, int64_t E,
-                                               const bool (&col_ok)[CH], int li, bool mean) {
+                                               const bool (&col_ok)[CH], int li, bool mean,
+                                               const uint8_t* __restrict__ res_row = nullptr, float rs = 0.f) {
     static_assert(VEC == 16 && std::is_same<T, float>::value, "e4m3 result: fp8 operand, fp32 accumulation");
+    static_assert(!RES || RED == R_SUM, "residual: sum / mean");
     float amax = 0.f;
 #pragma unroll
     for (int ch = 0; ch < CH; ch++) {
@@ -244,7 +253,12 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
         if (RED == R_SUM && mean) a = a / (float)(count > 0 ? count : 1);
         if (ARG && count == 0) a = 0.f;
         acc[ch * VEC + i] = a;
-        amax = amax_nan(amax, fabsf(a));
+        if constexpr (!RES) amax = amax_nan(amax, fabsf(a));
+      }
+      if constexpr (RES) {
+        res_add16(&acc[ch * VEC], res_row + (ch * LPR + li) * VEC, rs);
+#pragma unroll
+        for (int i = 0; i < VEC; i++) amax = amax_nan(amax, fabsf(acc[ch * VEC + i]));
       }
     }
     const unsigned gmask = LPR == 32 ? 0xffffffffu : (((1u << LPR) - 1u) << ((threadIdx.x & 31) & ~(LPR - 1)));
@@ -429,9 +443,11 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
     }
   }
 
+  template <bool RES = false>  // no residual with min / max
   __device__ __forceinline__ void store_row(T* __restrict__ out_row, int64_t* __restrict__ arg_row,
                                             int64_t count, int64_t E, const bool (&col_ok)[CH], int li, bool,
-                                            float* = nullptr, int = 0) {
+                                            float* = nullptr, int = 0, const uint8_t* = nullptr, float = 0.f) {
+    static_assert(!RES, "residual: sum / mean");
 #pragma unroll
     for (int ch = 0; ch < CH; ch++) {
       if (!col_ok[ch]) continue;
@@ -463,10 +479,11 @@ template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, cons
 }
 
 // column kk of a multi-segment row: its partials folded in segment order (min/max: the smallest e wins ties), the
-// mean's division applied. CG: read past L1 (partials written by other SMs during the same launch).
-template <int RED, bool CG>
+// mean's division applied. CG: read past L1 (partials written by other SMs during the same launch). RES: plus the
+// row's residual (scale rs) in that column.
+template <int RED, bool CG, bool RES = false>
 __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow& L, int nseg, int64_t count,
-                                             int64_t kk, int64_t& ar) {
+                                             int64_t kk, int64_t& ar, float rs = 0.f) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const float* pv = (const float*)p.part_val;
   float a = CG ? __ldcg(pv + L.first_slot * p.K + kk) : pv[L.first_slot * p.K + kk];
@@ -483,16 +500,18 @@ __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow&
     }
   }
   if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
+  if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
   return a;
 }
 
 // combine the partials of one multi-segment row, in segment order, by ONE WARP (planned mode: the warp that finished
-// the row's last segment); the partials were written by other SMs -> read them past L1
-template <typename T, int RED>
+// the row's last segment); the partials were written by other SMs -> read them past L1. RES: plus the residual.
+template <typename T, int RED, bool RES = false>
 __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const LongRow& L, int lane, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const int nseg = (int)(L.nseg_count >> 40);
   const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+  const float rs = RES ? res_scale(p, L.row_b) : 0.f;
   for (int k = lane; k < kcols; k += 32) {
     const int64_t kk = p.k0 + k;
     if (kk >= p.K) break;
@@ -508,23 +527,26 @@ __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const Long
       }
     }
     if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
+    if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
     ((T*)p.out)[L.row_b * p.K + kk] = Traits<T>::from_acc(a);
     if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
   }
 }
 
-// the same for an e4m3 result (QO): a first pass over the partials finds the row's amax, the second writes y / scale
-template <int RED>
+// the same for an e4m3 result (QO): a first pass over the partials finds the row's amax, the second writes y / scale.
+// RES: both passes add the residual, so the amax is taken over the values that are stored.
+template <int RED, bool RES = false>
 __device__ __forceinline__ void combine_row_warp_q8(const SpmmParams& p, const LongRow& L, int lane, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const int nseg = (int)(L.nseg_count >> 40);
   const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+  const float rs = RES ? res_scale(p, L.row_b) : 0.f;
   float amax = 0.f;
   for (int k = lane; k < kcols; k += 32) {
     const int64_t kk = p.k0 + k;
     if (kk >= p.K) break;
     int64_t ar;
-    amax = amax_nan(amax, fabsf(combine_col<RED, true>(p, L, nseg, count, kk, ar)));
+    amax = amax_nan(amax, fabsf(combine_col<RED, true, RES>(p, L, nseg, count, kk, ar, rs)));
   }
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
@@ -534,15 +556,15 @@ __device__ __forceinline__ void combine_row_warp_q8(const SpmmParams& p, const L
     const int64_t kk = p.k0 + k;
     if (kk >= p.K) break;
     int64_t ar;
-    const float a = combine_col<RED, true>(p, L, nseg, count, kk, ar);
+    const float a = combine_col<RED, true, RES>(p, L, nseg, count, kk, ar, rs);
     ((uint8_t*)p.out)[L.row_b * p.K + kk] = e4m3_quant(a, s);
     if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
   }
 }
 
-// QO: e4m3 result with per-row scales (RowEngine::store_row_q8) instead of T
+// QO: e4m3 result with per-row scales (RowEngine::store_row_q8) instead of T. RES: plus an e4m3 residual per row.
 template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
-          bool QO = false>
+          bool QO = false, bool RES = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_vec_kernel(const SpmmParams p) {
   using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
@@ -658,11 +680,14 @@ spmm_vec_kernel(const SpmmParams p) {
       eng.reduce_groups();
       if constexpr (QO) {
         if (g == 0)
-          eng.store_row_q8((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
-                           argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0);
+          eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
+                                         argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li,
+                                         p.mean != 0, RES ? res_row(p, r0 + rl) : nullptr,
+                                         RES ? res_scale(p, r0 + rl) : 0.f);
       } else {
-        if (g == 0) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
-                                  ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+        if (g == 0) eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
+                                  ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0,
+                                  RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
       }
     }
     item = __shfl_sync(0xffffffffu, next_item, 0);
@@ -692,12 +717,16 @@ spmm_vec_kernel(const SpmmParams p) {
       if (S.slot < 0) {
         if constexpr (QO) {
           if (g == 0)
-            eng.store_row_q8((uint8_t*)p.out + row * p.K, p.out_scale + row, p.arg_out ? p.arg_out + row * p.K : nullptr,
-                             S.end - S.start, p.E, col_ok, li, p.mean != 0);
+            eng.template store_row_q8<RES>((uint8_t*)p.out + row * p.K, p.out_scale + row,
+                                           p.arg_out ? p.arg_out + row * p.K : nullptr, S.end - S.start, p.E, col_ok,
+                                           li, p.mean != 0, RES ? res_row(p, row) : nullptr,
+                                           RES ? res_scale(p, row) : 0.f);
         } else {
           if (g == 0)
-            eng.store_row((T*)p.out + row * p.K + p.k0, p.arg_out ? p.arg_out + row * p.K + p.k0 : nullptr,
-                          S.end - S.start, p.E, col_ok, li, p.mean != 0);
+            eng.template store_row<RES>((T*)p.out + row * p.K + p.k0,
+                                        p.arg_out ? p.arg_out + row * p.K + p.k0 : nullptr, S.end - S.start, p.E,
+                                        col_ok, li, p.mean != 0, nullptr, 0, RES ? res_row(p, row) : nullptr,
+                                        RES ? res_scale(p, row) : 0.f);
         }
       } else {
         if (g == 0) {
@@ -723,8 +752,8 @@ spmm_vec_kernel(const SpmmParams p) {
         const LongRow L = p.longs[lr];
         if ((int)finished == (int)(L.nseg_count >> 40) - 1) {
           __threadfence();
-          if constexpr (QO) combine_row_warp_q8<RED>(p, L, lane, kcols);
-          else combine_row_warp<T, RED>(p, L, lane, kcols);
+          if constexpr (QO) combine_row_warp_q8<RED, RES>(p, L, lane, kcols);
+          else combine_row_warp<T, RED, RES>(p, L, lane, kcols);
         }
       }
       __syncwarp();
@@ -748,7 +777,7 @@ template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __
 }
 
 template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
-          bool QO = false>
+          bool QO = false, bool RES = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_gpr_kernel(const SpmmParams p) {
   using V = Vec<T>;
@@ -855,7 +884,6 @@ spmm_gpr_kernel(const SpmmParams p) {
       Eng eng;
       eng.init();
       set_scale(eng, p);
-
       // software pipeline: the (col, value) pairs of chunk k+1 are loaded while chunk k's gathers fly
       uint32_t cn[U];
       VR vn[U];
@@ -899,11 +927,14 @@ spmm_gpr_kernel(const SpmmParams p) {
       }
       if constexpr (QO) {  // `mine` is the same for the LPR lanes of a group, so the group's amax shuffle is complete
         if (mine)
-          eng.store_row_q8((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
-                           argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li, p.mean != 0);
+          eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
+                                         argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
+                                         p.mean != 0, RES ? res_row(p, r0 + rl) : nullptr,
+                                         RES ? res_scale(p, r0 + rl) : 0.f);
       } else {
-        if (mine) eng.store_row(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
-                                p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0);
+        if (mine) eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
+                                p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0,
+                                RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
       }
     }
     item = __shfl_sync(0xffffffffu, next_item, 0);
@@ -911,7 +942,8 @@ spmm_gpr_kernel(const SpmmParams p) {
 }
 
 // one warp per queued segment
-template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T, bool QO = false>
+template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T, bool QO = false,
+          bool RES = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_seg_kernel(const SpmmParams p) {
   using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
@@ -958,13 +990,16 @@ spmm_seg_kernel(const SpmmParams p) {
     if (g == 0) {
       if (S.slot < 0) {
         if constexpr (QO)
-          eng.store_row_q8((uint8_t*)p.out + row * p.K, p.out_scale + row, p.arg_out ? p.arg_out + row * p.K : nullptr,
-                           S.end - S.start, p.E, col_ok, li, p.mean != 0);
+          eng.template store_row_q8<RES>((uint8_t*)p.out + row * p.K, p.out_scale + row,
+                                         p.arg_out ? p.arg_out + row * p.K : nullptr, S.end - S.start, p.E, col_ok,
+                                         li, p.mean != 0, RES ? res_row(p, row) : nullptr,
+                                         RES ? res_scale(p, row) : 0.f);
         else
-          eng.store_row((T*)p.out + (b * p.M + row) * p.K + p.k0,
+          eng.template store_row<RES>((T*)p.out + (b * p.M + row) * p.K + p.k0,
                         p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
                         S.end - S.start, p.E, col_ok, li, p.mean != 0,
-                        ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0);
+                        ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0,
+                        RES ? res_row(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
       } else {
         float* pv = (float*)p.part_val + S.slot * p.K + p.k0;
         int64_t* pa = Eng::ARG ? p.part_arg + S.slot * p.K + p.k0 : nullptr;
@@ -984,8 +1019,8 @@ spmm_seg_kernel(const SpmmParams p) {
   }
 }
 
-// combine the partials of multi-segment rows, in segment order.
-template <typename T, int RED>
+// combine the partials of multi-segment rows, in segment order. RES: plus the residual, after the mean's division.
+template <typename T, int RED, bool RES = false>
 __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const int64_t nlong = p.plan_mask ? p.n_long : min((int64_t)p.counters[2], p.long_cap);
@@ -993,6 +1028,7 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
     const LongRow L = p.longs[li];
     const int nseg = (int)(L.nseg_count >> 40);
     const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+    const float rs = RES ? res_scale(p, L.row_b) : 0.f;
     for (int k = threadIdx.x; k < kcols; k += blockDim.x) {
       const int64_t kk = p.k0 + k;
       if (kk >= p.K) break;
@@ -1008,6 +1044,7 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
         }
       }
       if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
+      if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
       if (RED == R_SUM && p.acc_mode) {
         float* pr = p.partial + L.row_b * p.K + kk;
         if (p.acc_mode != 1) a += *pr;
@@ -1020,9 +1057,9 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
 }
 
 // the same for an e4m3 result (QO): per row, a first pass over the partials and a block reduction find the row's amax,
-// the second pass writes y / scale
+// the second pass writes y / scale. RES: both passes add the residual.
 constexpr int kCombineThreads = 128;
-template <int RED>
+template <int RED, bool RES = false>
 __global__ void __launch_bounds__(kCombineThreads) spmm_combine_q8_kernel(const SpmmParams p, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   __shared__ float s_amax[kCombineThreads / 32];
@@ -1031,12 +1068,13 @@ __global__ void __launch_bounds__(kCombineThreads) spmm_combine_q8_kernel(const 
     const LongRow L = p.longs[li];
     const int nseg = (int)(L.nseg_count >> 40);
     const int64_t count = L.nseg_count & (((int64_t)1 << 40) - 1);
+    const float rs = RES ? res_scale(p, L.row_b) : 0.f;
     float amax = 0.f;
     for (int k = threadIdx.x; k < kcols; k += kCombineThreads) {
       const int64_t kk = p.k0 + k;
       if (kk >= p.K) break;
       int64_t ar;
-      amax = amax_nan(amax, fabsf(combine_col<RED, false>(p, L, nseg, count, kk, ar)));
+      amax = amax_nan(amax, fabsf(combine_col<RED, false, RES>(p, L, nseg, count, kk, ar, rs)));
     }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
@@ -1051,7 +1089,7 @@ __global__ void __launch_bounds__(kCombineThreads) spmm_combine_q8_kernel(const 
       const int64_t kk = p.k0 + k;
       if (kk >= p.K) break;
       int64_t ar;
-      const float a = combine_col<RED, false>(p, L, nseg, count, kk, ar);
+      const float a = combine_col<RED, false, RES>(p, L, nseg, count, kk, ar, rs);
       ((uint8_t*)p.out)[L.row_b * p.K + kk] = e4m3_quant(a, s);
       if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
     }
@@ -1126,22 +1164,22 @@ static bool vec_eligible(int dtype, int64_t K, int64_t E, int64_t N, const void*
   return true;
 }
 
-template <typename T, int RED, bool QO>
+template <typename T, int RED, bool QO, bool RES = false>
 static void launch_combine(const SpmmParams& p, int kcols, cudaStream_t st) {
-  if constexpr (QO) spmm_combine_q8_kernel<RED><<<num_sms() * 2, kCombineThreads, 0, st>>>(p, kcols);
-  else spmm_combine_kernel<T, RED><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
+  if constexpr (QO) spmm_combine_q8_kernel<RED, RES><<<num_sms() * 2, kCombineThreads, 0, st>>>(p, kcols);
+  else spmm_combine_kernel<T, RED, RES><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
 }
 
 template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false,
-          typename X = T, bool QO = false>
+          typename X = T, bool QO = false, bool RES = false>
 static int launch_vec(SpmmParams p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(X);
   constexpr int kcols = LPR * CH * VEC;
   void (*kmain)(const SpmmParams);
-  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X, QO>;
-  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X, QO>;
+  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X, QO, RES>;
+  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X, QO, RES>;
   constexpr int USEG = (U > LPR) ? LPR : U;  // the row engine needs U * (32 / LPR) <= 32
-  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO>;
+  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO, RES>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   // small matrices: shrink the work item so that every resident warp gets rows
@@ -1167,7 +1205,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
         kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
         TSB_LAUNCH_CHECK();
         if (p.n_long > 0) {
-          launch_combine<T, RED, QO>(p, kcols, st);
+          launch_combine<T, RED, QO, RES>(p, kcols, st);
           TSB_LAUNCH_CHECK();
         }
       }
@@ -1179,7 +1217,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
       TSB_LAUNCH_CHECK();
       kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
       TSB_LAUNCH_CHECK();
-      launch_combine<T, RED, QO>(p, kcols, st);
+      launch_combine<T, RED, QO, RES>(p, kcols, st);
       TSB_LAUNCH_CHECK();
     }
   }
@@ -1189,7 +1227,8 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
 // (LPR, CH) follow from the width of a dense row; (U, MINB) = gathers in flight per lane and CTAs
 // per SM: the kernel is HBM-latency bound, so resident warps x gathers-in-flight wins (40 warps/SM x 4 x 16 B
 // per lane; the register budget of MINB = 5 is the same 64K registers per SM on sm_90).
-template <typename T, int RED, bool ACC = false, bool PLAN = false, typename X = T, bool QO = false>
+template <typename T, int RED, bool ACC = false, bool PLAN = false, typename X = T, bool QO = false,
+          bool RES = false>
 static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   // fp8 operand: a vector is 16 columns, so a lane keeps twice the accumulators (and arg slots) of a 16-bit operand
   // and needs more registers per thread: its own (U, CTAs/SM) per shape (ptxas report and times in DESIGN §3.1)
@@ -1199,33 +1238,40 @@ static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row
   // narrow rows: group-per-row kernel (all reductions)
   constexpr int GB = Q8 ? (MM ? 2 : 3) : 5;
-  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X, QO>(p, st);
-  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X, QO>(p, st);
-  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X, QO>(p, st);
-  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, GB, true, PLAN, X, QO>(p, st);
+  if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
+  if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
+  if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
+  if (vecs <= 8) return launch_vec<T, RED, ACC, 8, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
   // 256-byte rows (F = 128 bf16): at MINB = 5 the 48-register budget spills (120 B of stack in the planned kernel);
   // 3 CTAs/SM with 6 gathers in flight per lane is 8 % faster at C2 on the H100 (sweep in DESIGN §3.1)
   // e4m3 result (QO): the quantising epilogue (row amax, IEEE divisions) spills the sum kernels of 256-, 512- and
-  // 2048-byte rows at the CTAs/SM of the fp32 result; those take one CTA/SM less (ptxas table in DESIGN §3.1)
+  // 2048-byte rows at the CTAs/SM of the fp32 result; those take one CTA/SM less (ptxas table in DESIGN §3.1).
+  // A residual (RES) spills the planned kernels of the same shapes at that occupancy, so it takes the QO shapes.
+  constexpr bool LOW = MM || QO || RES;
   if (vecs <= 16)
-    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && (MM || QO) ? 2 : 3, false, PLAN, X, QO>(p, st);
+    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && LOW ? 2 : 3, false, PLAN, X, QO, RES>(p, st);
   if (vecs <= 32)
-    return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (MM || QO ? 2 : 3) : 5, false, PLAN, X, QO>(p, st);
-  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X, QO>(p, st);
+    return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (LOW ? 2 : 3) : 5, false, PLAN, X, QO, RES>(p, st);
+  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X, QO, RES>(p, st);
   // column-tiled beyond 128 vectors
-  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (MM || QO ? 1 : 2) : 3, false, PLAN, X, QO>(p, st);
+  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (LOW ? 1 : 2) : 3, false, PLAN, X, QO, RES>(p, st);
 }
 
-template <typename T, bool PLAN = false, typename X = T, bool QO = false>
+template <typename T, bool PLAN = false, typename X = T, bool QO = false, bool RES = false>
 static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
   p.mean = (reduce == TSB200_MEAN);
-  switch (reduce) {
-    case TSB200_SUM:
-    case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN, X, QO>(p, st);
-    case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN, X, QO>(p, st);
-    case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN, X, QO>(p, st);
+  if constexpr (RES) {  // a residual is added to sums and means only
+    if (reduce != TSB200_SUM && reduce != TSB200_MEAN) return TSB200_ERR_UNSUPPORTED;
+    return dispatch_shape<T, R_SUM, false, PLAN, X, QO, true>(p, st);
+  } else {
+    switch (reduce) {
+      case TSB200_SUM:
+      case TSB200_MEAN: return dispatch_shape<T, R_SUM, false, PLAN, X, QO>(p, st);
+      case TSB200_MIN: return dispatch_shape<T, R_MIN, false, PLAN, X, QO>(p, st);
+      case TSB200_MAX: return dispatch_shape<T, R_MAX, false, PLAN, X, QO>(p, st);
+    }
+    return TSB200_ERR_INVALID_ARG;
   }
-  return TSB200_ERR_INVALID_ARG;
 }
 
 // ---- plan: the segment list of a matrix, built once (tsb200_spmm_plan) -----------------------------------------
@@ -1516,20 +1562,58 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
 // ---- SpMM over an fp8 (e4m3) dense operand with per-tensor or per-row scales ----------------------------------------
 // The same kernels, instantiated with X = __nv_fp8_e4m3: value / output type T = out_dtype, a dense row is K bytes.
 // out_scale != NULL: e4m3 result with per-row scales (tsb200_spmm_fw_fp8_quant): T = float, `out` is e4m3 [M, K].
+// res8 != NULL: plus an e4m3 residual with its own scales (tsb200_spmm_fw_fp8_res): the RES instantiations, sum / mean.
 namespace tsb {
 __global__ void fill_f32_kernel(float* __restrict__ p, int64_t n, float v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
-template <bool PLAN, bool QO>
+// An empty matrix with a residual: every row is y = +0, so the result is z = fl32(+0 + rho) (a -0 residual gives +0).
+// One warp per row; an e4m3 result takes the row amax of z first (K <= 2048), then writes z / scale.
+template <typename T, bool QO>
+__global__ void __launch_bounds__(256) spmm_res_only_kernel(const SpmmParams p) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t m = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; m < p.M; m += nw) {
+    const float rs = res_scale(p, m);
+    const uint8_t* r = p.res8 + m * p.K;
+    if constexpr (QO) {
+      float amax = 0.f;
+      for (int64_t k = lane; k < p.K; k += 32) amax = amax_nan(amax, fabsf(res_add(0.f, rs, __ldcs(r + k))));
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+      const float s = e4m3_row_scale(amax);
+      if (lane == 0) p.out_scale[m] = s;
+      for (int64_t k = lane; k < p.K; k += 32) ((uint8_t*)p.out)[m * p.K + k] = e4m3_quant(res_add(0.f, rs, r[k]), s);
+    } else {
+      for (int64_t k = lane; k < p.K; k += 32)
+        ((T*)p.out)[m * p.K + k] = Traits<T>::from_acc(res_add(0.f, rs, __ldcs(r + k)));
+    }
+  }
+}
+
+template <bool PLAN, bool QO, bool RES = false>
 static int dispatch_fp8_out(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
-  if constexpr (QO) return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, true>(p, reduce, st);
+  if constexpr (QO) return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, true, RES>(p, reduce, st);
   switch (out_dtype) {
-    case TSB200_F32: return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3>(p, reduce, st);
-    case TSB200_F16: return dispatch_red_vec<__half, PLAN, __nv_fp8_e4m3>(p, reduce, st);
-    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, PLAN, __nv_fp8_e4m3>(p, reduce, st);
+    case TSB200_F32: return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
+    case TSB200_F16: return dispatch_red_vec<__half, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
+    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
   }
   return TSB200_ERR_UNSUPPORTED;
+}
+template <bool PLAN, bool QO>
+static int dispatch_fp8_res(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
+  if (p.res8) return dispatch_fp8_out<PLAN, QO, true>(p, out_dtype, reduce, st);
+  return dispatch_fp8_out<PLAN, QO>(p, out_dtype, reduce, st);
+}
+
+template <typename T, bool QO>
+static int launch_res_only(const SpmmParams& p, cudaStream_t st) {
+  const int64_t blocks = min((p.M * 32 + 255) / 256, (int64_t)num_sms() * 16);
+  spmm_res_only_kernel<T, QO><<<(int)blocks, 256, 0, st>>>(p);
+  TSB_LAUNCH_CHECK();
+  return 0;
 }
 
 template <bool QO>
@@ -1537,7 +1621,8 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
                             const float* scale, int64_t scale_stride, void* out, float* out_scale, int64_t* arg_out,
                             int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
                             size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
-                            size_t workspace_bytes, void* stream) {
+                            size_t workspace_bytes, void* stream, const uint8_t* res8 = nullptr,
+                            const float* res_scale = nullptr, int64_t res_stride = 0) {
   if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
   if (reduce < TSB200_SUM || reduce > TSB200_MAX) return TSB200_ERR_INVALID_ARG;
   if (scale_stride != 0 && scale_stride != 1) return TSB200_ERR_INVALID_ARG;
@@ -1550,6 +1635,24 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
   if (!rowptr || !out || (QO && !out_scale) || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
   if (QO && ((uintptr_t)out_scale & 3)) return TSB200_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
+  SpmmParams p;
+  p.res8 = res8; p.res_scale = res_scale; p.res_stride = (uint32_t)res_stride;
+  if (res8) {
+    if (!res_scale || (res_stride != 0 && res_stride != 1)) return TSB200_ERR_INVALID_ARG;
+    if (arg) return TSB200_ERR_UNSUPPORTED;
+    if (((uintptr_t)res8 & 15) || ((uintptr_t)res_scale & 3)) return TSB200_ERR_UNSUPPORTED;
+    if (E == 0 && K > 0) {  // every row is empty: the result is the residual alone
+      if ((uintptr_t)out & 15) return TSB200_ERR_UNSUPPORTED;
+      p.out = out; p.out_scale = out_scale; p.M = M; p.K = K; p.k0 = 0;
+      if constexpr (QO) return launch_res_only<float, true>(p, st);
+      switch (out_dtype) {
+        case TSB200_F32: return launch_res_only<float, false>(p, st);
+        case TSB200_F16: return launch_res_only<__half, false>(p, st);
+        case TSB200_BF16: return launch_res_only<__nv_bfloat16, false>(p, st);
+      }
+      return TSB200_ERR_UNSUPPORTED;
+    }
+  }
   if (E == 0 || K == 0) {  // every row is empty: 0, arg_out = E = 0, and a scale of 1 (an amax of 0)
     if (K > 0) {
       TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(M * K) * (QO ? 1 : dtype_size(out_dtype)), st));
@@ -1568,7 +1671,6 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
   if ((value && ((uintptr_t)value & 3)) || (arg_out && ((uintptr_t)arg_out & 15))) return TSB200_ERR_UNSUPPORTED;
   if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
   char* ws = (char*)workspace;
-  SpmmParams p;
   p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
   p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
   p.partial = nullptr; p.acc_mode = 0;
@@ -1591,7 +1693,7 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
     p.part_val = ws + W.part_val;
     p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
     p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
-    return dispatch_fp8_out<true, QO>(p, out_dtype, reduce, st);
+    return dispatch_fp8_res<true, QO>(p, out_dtype, reduce, st);
   }
   // unplanned: the layout of tsb200_spmm_fw (tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce))
   const WsLayout L = ws_layout(1, K, E, arg);
@@ -1603,7 +1705,7 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
   p.part_val = ws + L.part_val;
   p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
   p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
-  return dispatch_fp8_out<false, QO>(p, out_dtype, reduce, st);
+  return dispatch_fp8_res<false, QO>(p, out_dtype, reduce, st);
 }
 }  // namespace tsb
 
@@ -1625,4 +1727,21 @@ extern "C" int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* co
   return spmm_fw_fp8_impl<true>(rowptr, col, value, mat, scale, scale_stride, out8, out_scale, arg_out, M, N, K, E,
                                 TSB200_F32, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace,
                                 workspace_bytes, stream);
+}
+
+extern "C" int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                      const float* scale, int64_t scale_stride, const void* res8,
+                                      const float* res_scale, int64_t res_scale_stride, void* out, float* out_scale,
+                                      int64_t* arg_out, int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype,
+                                      int reduce, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                                      int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream) {
+  if (out_scale) {
+    if (out_dtype != TSB200_F32) return TSB200_ERR_INVALID_ARG;  // an e4m3 result takes float32 values
+    return spmm_fw_fp8_impl<true>(rowptr, col, value, mat, scale, scale_stride, out, out_scale, arg_out, M, N, K, E,
+                                  TSB200_F32, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace,
+                                  workspace_bytes, stream, (const uint8_t*)res8, res_scale, res_scale_stride);
+  }
+  return spmm_fw_fp8_impl<false>(rowptr, col, value, mat, scale, scale_stride, out, nullptr, arg_out, M, N, K, E,
+                                 out_dtype, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes,
+                                 stream, (const uint8_t*)res8, res_scale, res_scale_stride);
 }

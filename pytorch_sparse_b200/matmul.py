@@ -81,11 +81,14 @@ def spmm(src: SparseTensor, other: Tensor, reduce: str = "sum") -> Tensor:
 
 
 def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
-             out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
+             out_dtype: torch.dtype = torch.bfloat16, residual: Optional[Tensor] = None,
+             residual_scale: Optional[Tensor] = None) -> Tensor:
     """`src @ (x8 * scale)` over an FP8 (e4m3) dense operand `x8` [N, K] (K % 16 == 0) with a float32 `scale` of
     shape [] or [N] (see `quantize_fp8`), reduce in sum/add/mean/min/max, result in `out_dtype` (bf16, f16, f32).
     The entry values are cast to `out_dtype` first, as `spmm` casts them to the dense dtype. Forward only: no
-    gradient flows, and a `value` or `scale` that requires grad is refused while grad mode is on."""
+    gradient flows, and a `value` or `scale` that requires grad is refused while grad mode is on.
+    With `residual` (e4m3 [M, K]) and `residual_scale` (float32 [] or [M]), sum / mean only, the kernel adds
+    `residual_scale[m] * residual[m]` to row m of the float32 result before rounding it to `out_dtype`."""
     rowptr, col, value = src.csr()
     if value is not None:
         value = value.to(out_dtype)
@@ -93,15 +96,20 @@ def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
         reduce = "sum"
     if reduce != "sum" and reduce != "mean" and reduce != "min" and reduce != "max":
         raise ValueError("unknown reduce '" + reduce + "'")
-    return torch.ops.tsb200.spmm_fp8(rowptr, col, value, x8, scale, reduce, out_dtype)[0]
+    return torch.ops.tsb200.spmm_fp8(rowptr, col, value, x8, scale, reduce, out_dtype, residual, residual_scale)[0]
 
 
-def spmm_fp8_quant(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum") -> Tuple[Tensor, Tensor]:
+def spmm_fp8_quant(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
+                   residual: Optional[Tensor] = None, residual_scale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """One FP8 propagation hop: `src @ (x8 * scale)` as `spmm_fp8(..., torch.float32)` computes it, returned as
     `(y8, y_scale)` = `quantize_fp8(y, per_row=True)` of that float32 result, bit for bit, without materialising y:
     the kernels quantise each row as they store it. The pair is the `x8` / `scale` of the next hop, so repeated
     propagation (SIGN, APPNP, label propagation) stays in e4m3. K <= 2048 columns; entry values are cast to float32.
-    Forward only: a `value` or `scale` that requires grad is refused while grad mode is on."""
+    Forward only: a `value` or `scale` that requires grad is refused while grad mode is on.
+    With `residual` (e4m3 [M, K]) and `residual_scale` (float32 [] or [M]), sum / mean only, the rows quantised are
+    `y[m] + residual_scale[m] * residual[m]` (one fp32 product and one fp32 add), so a propagation step with a fixed
+    residual term stays in e4m3: APPNP `X = (1 - a) A X + a H` takes entry values times (1 - a) and `residual_scale`
+    times a (see README)."""
     rowptr, col, value = src.csr()
     if value is not None:
         value = value.to(torch.float32)
@@ -109,7 +117,7 @@ def spmm_fp8_quant(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "
         reduce = "sum"
     if reduce != "sum" and reduce != "mean" and reduce != "min" and reduce != "max":
         raise ValueError("unknown reduce '" + reduce + "'")
-    y8, y_scale, _ = torch.ops.tsb200.spmm_fp8_quant(rowptr, col, value, x8, scale, reduce)
+    y8, y_scale, _ = torch.ops.tsb200.spmm_fp8_quant(rowptr, col, value, x8, scale, reduce, residual, residual_scale)
     return y8, y_scale
 
 
@@ -180,9 +188,10 @@ def matmul(src, other, reduce="sum"):  # noqa: F811
 
 
 SparseTensor.spmm = lambda self, other, reduce="sum": spmm(self, other, reduce)
-SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bfloat16: spmm_fp8(
-    self, x8, scale, reduce, out_dtype)
-SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum": spmm_fp8_quant(self, x8, scale, reduce)
+SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bfloat16, residual=None, \
+    residual_scale=None: spmm_fp8(self, x8, scale, reduce, out_dtype, residual, residual_scale)
+SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum", residual=None, residual_scale=None: spmm_fp8_quant(
+    self, x8, scale, reduce, residual, residual_scale)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)
 SparseTensor.__matmul__ = lambda self, other: matmul(self, other, "sum")

@@ -257,6 +257,64 @@ def _fp8_args(what: str, rowptr: Tensor, col: Tensor, value: Optional[Tensor], x
     return _i64(rowptr, "rowptr"), _i64(col, "col"), value, scale, stride
 
 
+def _fp8_residual(what: str, residual: Optional[Tensor], residual_scale: Optional[Tensor], x8: Tensor, M: int,
+                  red: int):
+    """The checks of the optional residual of spmm_fw_fp8 / spmm_fw_fp8_quant: None without one, otherwise
+    (residual, residual_scale, residual_scale_stride)."""
+    if residual is None and residual_scale is None:
+        return None
+    if residual is None or residual_scale is None:
+        raise RuntimeError(f"{what}: residual and residual_scale go together: pass both or neither")
+    _check_cuda(residual, "residual")
+    _check_cuda(residual_scale, "residual_scale")
+    if red >= 2:
+        raise RuntimeError(f"{what}: a residual is only added to reduce='sum' / 'mean' results, not min / max")
+    if torch.is_grad_enabled() and residual_scale.requires_grad:
+        raise RuntimeError(f"{what} is forward only: residual_scale must not require grad "
+                           "(call it under torch.no_grad() or detach it)")
+    if residual.device != x8.device or residual_scale.device != x8.device:
+        raise RuntimeError(f"{what}: residual and residual_scale must be on the device of x8 ({x8.device})")
+    if residual.dtype != torch.float8_e4m3fn:
+        raise RuntimeError(f"{what}: residual must be torch.float8_e4m3fn, got {residual.dtype}")
+    K = x8.size(1)
+    if residual.dim() != 2 or residual.size(0) != M or residual.size(1) != K:
+        raise RuntimeError(f"{what}: residual must have the result's shape [M, K] = [{M}, {K}], "
+                           f"got {list(residual.shape)}")
+    if not residual.is_contiguous() or residual.data_ptr() % 16 != 0:
+        raise RuntimeError(f"{what}: residual must be contiguous and 16-byte aligned")
+    if residual_scale.dtype != torch.float32:
+        raise RuntimeError(f"{what}: residual_scale must be float32, got {residual_scale.dtype}")
+    if residual_scale.dim() == 0:
+        stride = 0
+    elif residual_scale.dim() == 1 and residual_scale.size(0) == M:
+        stride = 1
+    else:
+        raise RuntimeError(f"{what}: residual_scale must have shape [] or [M] = [{M}], "
+                           f"got {list(residual_scale.shape)}")
+    return residual, residual_scale.contiguous(), stride
+
+
+def _fp8_res_call(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor, stride: int, res,
+                  out: Tensor, out_scale: Optional[Tensor], dt: int, red: int, plan: Optional[SpmmPlan]) -> None:
+    """tsb200_spmm_fw_fp8_res: out_dtype code `dt` result, or an e4m3 result when out_scale is given (dt = float32)."""
+    residual, residual_scale, rstride = res
+    N, K = x8.shape
+    M, E = rowptr.numel() - 1, col.numel()
+    dev = x8.device
+    with _on_device(dev):
+        plan = _fp8_plan(plan, rowptr, M, E) if E > 0 else None
+        if plan is not None:
+            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
+            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
+        else:
+            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, dt, red)
+            pl, pl_bytes, counts = None, 0, (0, 0, 0)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_fw_fp8_res(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(residual),
+                                         _p(residual_scale), rstride, _p(out), _p(out_scale), None, M, N, K, E, dt, red,
+                                         pl, pl_bytes, *counts, _p(ws), nws, _stream(dev)), "tsb200_spmm_fw_fp8_res")
+
+
 def _fp8_plan(plan: Optional[SpmmPlan], rowptr: Tensor, M: int, E: int) -> Optional[SpmmPlan]:
     if plan is None:
         plan = _auto_plan(rowptr, E)
@@ -267,21 +325,28 @@ def _fp8_plan(plan: Optional[SpmmPlan], rowptr: Tensor, M: int, E: int) -> Optio
 
 def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
                 reduce: str = "sum", out_dtype: torch.dtype = torch.bfloat16,
-                plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor]]:
+                plan: Optional[SpmmPlan] = None, residual: Optional[Tensor] = None,
+                residual_scale: Optional[Tensor] = None) -> Tuple[Tensor, Optional[Tensor]]:
     """`spmm_fw_fp8(rowptr, col, optional_value, x8, scale, reduce, out_dtype) -> (out, arg_out?)`
     (tsb200_spmm_fw_fp8): the SpMM forward over an e4m3 dense operand `x8` [N, K] (K % 16 == 0) whose row c stands for
     `x8[c].float() * scale[c]` (`scale` float32 of shape [N]) or `x8[c].float() * scale` (shape []). `value` has
     `out_dtype` (bf16, f16 or f32), as `spmm_fw`'s value has the dense dtype. Entry e weighs fl32(value[e] * scale[c]);
     sums accumulate weight * x8 in fp32 and round once, min/max compare the product rounded to `out_dtype`. Forward
-    only. Planned like `spmm_fw` (the same per-rowptr plan cache)."""
+    only. Planned like `spmm_fw` (the same per-rowptr plan cache).
+    `residual` (e4m3 [M, K]) with `residual_scale` (float32 [] or [M]), sum / mean only (tsb200_spmm_fw_fp8_res): the
+    result is round_out(fl32(y + fl32(residual_scale[m] * residual[m]))) with y the float32 result."""
     rowptr, col, value, scale, stride = _fp8_args("spmm_fp8", rowptr, col, value, x8, scale, out_dtype)
     red = _reduce_code(reduce)
     N, K = x8.shape
     M, E = rowptr.numel() - 1, col.numel()
+    res = _fp8_residual("spmm_fp8", residual, residual_scale, x8, M, red)
     dev = x8.device
     out = torch.empty(M, K, dtype=out_dtype, device=dev)
     arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
     if out.numel() == 0:
+        return out, arg_out
+    if res is not None:
+        _fp8_res_call(rowptr, col, value, x8, scale, stride, res, out, None, _FP8_OUT[out_dtype], red, plan)
         return out, arg_out
     if E == 0:
         out.zero_()
@@ -307,24 +372,30 @@ FP8_QUANT_MAX_K = 2048
 
 
 def spmm_fw_fp8_quant(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
-                      reduce: str = "sum",
-                      plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Tensor, Optional[Tensor]]:
+                      reduce: str = "sum", plan: Optional[SpmmPlan] = None, residual: Optional[Tensor] = None,
+                      residual_scale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor, Optional[Tensor]]:
     """`spmm_fw_fp8_quant(rowptr, col, optional_value, x8, scale, reduce) -> (y8, y_scale, arg_out?)`
     (tsb200_spmm_fw_fp8_quant): `spmm_fw_fp8` with a float32 result y, written as e4m3 with one scale per row by the
     kernel itself: y_scale[m] = amax|y[m]| / 448 (1 when that is not > 0, NaN rows included) and y8 = e4m3(y / y_scale),
     bit for bit `quantize_fp8(y, per_row=True)` on the CPU. `value` is float32. (y8, y_scale) are the `x8` and `scale`
-    of the next hop. K <= 2048. Forward only; planned like `spmm_fw` (the same per-rowptr plan cache)."""
+    of the next hop. K <= 2048. Forward only; planned like `spmm_fw` (the same per-rowptr plan cache).
+    `residual` (e4m3 [M, K]) with `residual_scale` (float32 [] or [M]), sum / mean only (tsb200_spmm_fw_fp8_res):
+    the rows quantised are z = fl32(y + fl32(residual_scale[m] * residual[m])) instead of y."""
     rowptr, col, value, scale, stride = _fp8_args("spmm_fp8_quant", rowptr, col, value, x8, scale, None)
     N, K = x8.shape
     if K > FP8_QUANT_MAX_K:
         raise RuntimeError(f"spmm_fp8_quant: the number of columns K = {K} must be at most {FP8_QUANT_MAX_K}")
     red = _reduce_code(reduce)
     M, E = rowptr.numel() - 1, col.numel()
+    res = _fp8_residual("spmm_fp8_quant", residual, residual_scale, x8, M, red)
     dev = x8.device
     y8 = torch.empty(M, K, dtype=torch.float8_e4m3fn, device=dev)
     y_scale = torch.empty(M, dtype=torch.float32, device=dev)
     arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
     if M == 0:
+        return y8, y_scale, arg_out
+    if res is not None and K > 0:
+        _fp8_res_call(rowptr, col, value, x8, scale, stride, res, y8, y_scale, _FP8_OUT[torch.float32], red, plan)
         return y8, y_scale, arg_out
     if E == 0 or K == 0:
         y8.zero_()

@@ -43,10 +43,11 @@ _EXTRA_SCHEMAS = {
     "segment_reduce": "(Tensor ptr, Tensor value, str reduce, Tensor? perm, Tensor? seg) -> Tensor",
     "spspmm": "(Tensor rowptrA, Tensor colA, Tensor? valueA, Tensor rowptrB, Tensor colB, Tensor? valueB, "
               "int M, int K, int N, bool want_value) -> (Tensor, Tensor, Tensor, Tensor?)",
+    # residual / residual_scale: an e4m3 residual added to every row (sum / mean; tsb200_spmm_fw_fp8_res)
     "spmm_fp8": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
-                "ScalarType out_dtype) -> (Tensor, Tensor?)",
-    "spmm_fp8_quant": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce) "
-                      "-> (Tensor, Tensor, Tensor?)",
+                "ScalarType out_dtype, Tensor? residual=None, Tensor? residual_scale=None) -> (Tensor, Tensor?)",
+    "spmm_fp8_quant": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
+                      "Tensor? residual=None, Tensor? residual_scale=None) -> (Tensor, Tensor, Tensor?)",
 }
 
 
@@ -60,10 +61,11 @@ _EXTRA_IMPLS = {
     "coalesce": ops.coalesce, "sort_perm": ops.sort_perm, "csr2csc": _csr2csc,
     "segment_reduce": lambda ptr, value, reduce, perm, seg: ops.segment_reduce(ptr, value, reduce, perm, seg),
     "spspmm": ops.spspmm,
-    "spmm_fp8": lambda rowptr, col, value, x8, scale, reduce, out_dtype: ops.spmm_fw_fp8(rowptr, col, value, x8, scale,
-                                                                                         reduce, out_dtype),
-    "spmm_fp8_quant": lambda rowptr, col, value, x8, scale, reduce: ops.spmm_fw_fp8_quant(rowptr, col, value, x8,
-                                                                                          scale, reduce),
+    "spmm_fp8": lambda rowptr, col, value, x8, scale, reduce, out_dtype, residual=None, residual_scale=None:
+        ops.spmm_fw_fp8(rowptr, col, value, x8, scale, reduce, out_dtype, residual=residual,
+                        residual_scale=residual_scale),
+    "spmm_fp8_quant": lambda rowptr, col, value, x8, scale, reduce, residual=None, residual_scale=None:
+        ops.spmm_fw_fp8_quant(rowptr, col, value, x8, scale, reduce, residual=residual, residual_scale=residual_scale),
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

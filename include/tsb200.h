@@ -184,6 +184,32 @@ TSB200_API int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col,
                                       int reduce, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
                                       int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * FP8 (e4m3) quantisation of a float matrix: the operand of tsb200_spmm_fw_fp8, made without float temporaries (no
+ * counterpart in the reference).
+ *   x dtype[N, K] with dtype in {F32, F16, BF16}, row m at x + m * ld elements (ld >= K; the last dimension is
+ *   contiguous, so a column slice of a wider matrix needs no copy). Per row (per_row = 1) or over the whole tensor
+ *   (per_row = 0), with xf = fl32(x) (exact):
+ *     amax  = max |xf|, NaN if any element is NaN;
+ *     scale = amax / 448 (IEEE fp32 division) when amax > 0, otherwise 1 (all-zero, all -0 and NaN rows);
+ *     x8    = e4m3(xf / scale) (IEEE division), rounded as torch's non-saturating float8_e4m3fn cast: nearest even,
+ *             subnormals kept, -0 stays -0, |q| > 464 and +-inf become NaN (an inf row gets scale inf).
+ *   That is, bit for bit, torch's quantize_fp8(x, per_row) on the CPU (NaN in any encoding), and the rounding of
+ *   tsb200_spmm_fw_fp8_quant's e4m3 result.
+ *   x8 e4m3[N, K] contiguous; scale f32[N] (per row) or f32[1] (per tensor), 4-byte aligned.
+ *   Rows are read with 16-byte loads when x, ld * size and K * size are multiples of 16 bytes and x8 is 16-byte
+ *   aligned, element by element otherwise; both give the same bits.
+ *   workspace: per_row = 0 only, >= 4 bytes, 4-byte aligned (one amax word; the call clears it); may be NULL per row.
+ *   No host synchronisation (CUDA-graph capturable): per row one kernel, per tensor a memset, an amax kernel and the
+ *   quantise kernel.
+ *   N == 0 per row: nothing is launched. TSB200_ERR_INVALID_ARG for a negative extent, ld < K, per_row not 0 / 1,
+ *   NULL x / x8 / scale, K == 0 or (per tensor) N == 0 (the amax of no elements); TSB200_ERR_UNSUPPORTED for another
+ *   dtype, K >= 2^31, or a misaligned x (element size), scale or workspace; TSB200_ERR_WORKSPACE for a missing or
+ *   short per-tensor workspace.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_quantize_fp8(const void* x, int64_t N, int64_t K, int64_t ld, int dtype, int per_row, void* x8,
+                                   float* scale, void* workspace, size_t workspace_bytes, void* stream);
+
 /* One COLUMN BLOCK of a SUM SpMM (multi-GPU pipelining: the dense operand arrives block by block over NVLink and
  * block p of A's columns is multiplied as soon as block p of `mat` has landed; no counterpart in the reference, which
  * has no collectives — the partitioner semantics are torch_sparse/narrow.py:15-42). (rowptr, col, value) hold only the

@@ -123,10 +123,19 @@ def spmm_fp8_quant(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "
 
 def quantize_fp8(x: Tensor, per_row: bool = True) -> Tuple[Tensor, Tensor]:
     """A 2-D floating `x` [N, K] as `(x8, scale)` for `spmm_fp8`: scale = amax|x| / 448 (e4m3's largest finite value)
-    per row ([N]) or over the whole tensor ([]), 1 where that amax is 0, and x8 = e4m3(x / scale), rounded to
-    nearest. Pure torch, on the device of `x`."""
+    per row ([N]) or over the whole tensor ([]), 1 where that amax is not > 0 (all-zero and NaN rows), and
+    x8 = e4m3(x.float() / scale), rounded to nearest even; magnitudes past 464 and inf become NaN.
+    A CUDA `x` is quantised by one streaming kernel (`torch.ops.tsb200.quantize_fp8`, two launches for a per-tensor
+    scale) without float temporaries, bit for bit the CPU result; bf16, f16 and f32 are read as they are, other dtypes
+    through `.float()`, and a column slice of a wider matrix is read in place. The torch expression below is the
+    definition: it runs for a CPU `x`, and for an `x` that requires grad while grad mode is on, whose `scale` keeps
+    its autograd history."""
     if x.dim() != 2:
         raise ValueError("quantize_fp8 expects a 2-D tensor [N, K]")
+    if x.is_cuda and not (x.requires_grad and torch.is_grad_enabled()):
+        if x.dtype != torch.bfloat16 and x.dtype != torch.float16 and x.dtype != torch.float32:
+            x = x.float()
+        return torch.ops.tsb200.quantize_fp8(x, per_row)
     xf = x.float()
     amax = xf.abs().amax(dim=1) if per_row else xf.abs().amax()
     scale = torch.where(amax > 0, amax / 448.0, torch.ones_like(amax))

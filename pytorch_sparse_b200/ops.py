@@ -418,6 +418,46 @@ def spmm_fw_fp8_quant(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: 
     return y8, y_scale, arg_out
 
 
+_QUANT_IN = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
+# torch's own messages for the amax of no elements, which the CPU quantize_fp8 raises
+_AMAX_EMPTY_DIM = "amax(): Expected reduction dim 1 to have non-zero size."
+_AMAX_EMPTY = ("amax(): Expected reduction dim to be specified for input.numel() == 0. "
+               "Specify the reduction dim with the 'dim' argument.")
+
+
+def quantize_fp8(x: Tensor, per_row: bool = True) -> Tuple[Tensor, Tensor]:
+    """`quantize_fp8(x, per_row) -> (x8, scale)` (tsb200_quantize_fp8): a bf16 / f16 / f32 CUDA matrix [N, K] as e4m3
+    with a float32 scale per row ([N]) or for the whole tensor ([]), bit for bit `matmul.quantize_fp8(x.cpu())`:
+    scale = amax|x| / 448 (IEEE division), 1 when that amax is not > 0 (NaN included), x8 = e4m3(x / scale). One
+    streaming kernel (two for a per-tensor scale) and no float temporaries; rows may be strided (`x[:, a:b]` of a
+    wider matrix is read in place), a last dimension that is not contiguous is copied first. x8 is contiguous and
+    16-byte aligned, a valid `spmm_fp8` operand. No host synchronisation, so the call can be captured in a CUDA graph.
+    Forward only: the outputs carry no autograd history."""
+    _check_cuda(x, "x")
+    if x.dim() != 2:
+        raise ValueError("quantize_fp8 expects a 2-D tensor [N, K]")
+    if x.dtype not in _QUANT_IN:
+        raise RuntimeError(f"quantize_fp8: x must be torch.bfloat16, torch.float16 or torch.float32, got {x.dtype}")
+    N, K = x.shape
+    if K == 0:
+        raise IndexError(_AMAX_EMPTY_DIM) if per_row else RuntimeError(_AMAX_EMPTY)
+    if N == 0 and not per_row:
+        raise RuntimeError(_AMAX_EMPTY)
+    if (K > 1 and x.stride(1) != 1) or (N > 1 and x.stride(0) < K):
+        x = x.contiguous()
+    ld = x.stride(0) if N > 1 else K
+    dev = x.device
+    x8 = torch.empty(N, K, dtype=torch.float8_e4m3fn, device=dev)
+    scale = torch.empty((N,) if per_row else (), dtype=torch.float32, device=dev)
+    if N == 0:
+        return x8, scale
+    ws = None if per_row else torch.empty(4, dtype=torch.uint8, device=dev)   # the per-tensor amax word
+    with _on_device(dev):
+        check(lib.tsb200_quantize_fp8(_p(x), N, K, ld, _QUANT_IN[x.dtype], int(per_row), _p(x8), _p(scale), _p(ws),
+                                      0 if ws is None else ws.numel(), _stream(dev)), "tsb200_quantize_fp8")
+    return x8, scale
+
+
 def spmm_fw_acc(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, partial: Tensor,
                 out: Optional[Tensor], acc_mode: int) -> None:
     """One column block of a SUM SpMM whose blocks are launched separately (tsb200_spmm_fw_acc): `partial` is the

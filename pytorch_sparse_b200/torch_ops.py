@@ -2,7 +2,8 @@
 (csrc/spmm.cpp:305-348, csrc/convert.cpp:46-48):
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
-    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant}  (own additions)
+    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant,
+                      quantize_fp8}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -48,6 +49,7 @@ _EXTRA_SCHEMAS = {
                 "ScalarType out_dtype, Tensor? residual=None, Tensor? residual_scale=None) -> (Tensor, Tensor?)",
     "spmm_fp8_quant": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
                       "Tensor? residual=None, Tensor? residual_scale=None) -> (Tensor, Tensor, Tensor?)",
+    "quantize_fp8": "(Tensor x, bool per_row) -> (Tensor, Tensor)",
 }
 
 
@@ -66,6 +68,7 @@ _EXTRA_IMPLS = {
                         residual_scale=residual_scale),
     "spmm_fp8_quant": lambda rowptr, col, value, x8, scale, reduce, residual=None, residual_scale=None:
         ops.spmm_fw_fp8_quant(rowptr, col, value, x8, scale, reduce, residual=residual, residual_scale=residual_scale),
+    "quantize_fp8": ops.quantize_fp8,
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -2,7 +2,7 @@
 
     a  bf16 -> bf16          ops.spmm_fw(rowptr, col, value_bf16, x_bf16, "sum", plan)
     b  fp8 -> bf16           ops.spmm_fw_fp8(..., x8, scale [N], "sum", bf16, plan)
-    c  b, then quantize_fp8  the e4m3 operand of the next hop through a float copy (pure torch)
+    c  b, then quantize_fp8  the e4m3 operand of the next hop from the bf16 result
     d  fp8 -> fp8            ops.spmm_fw_fp8_quant(..., x8, scale [N], "sum", plan): quantised in the kernel epilogue
 
 The variants alternate within one job (ROUNDS rounds of CALLS timed calls each, CUDA events); each round's ms per hop

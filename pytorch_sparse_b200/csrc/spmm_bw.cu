@@ -346,6 +346,8 @@ static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t 
   int64_t want = p.M / ((int64_t)grid_main * kWarpsPerCta * 2);
   p.item_shift = 0;
   while (p.item_shift < 5 && ((int64_t)2 << p.item_shift) <= want) p.item_shift++;
+  const int forced_shift = item_shift_override();  // tests: every item size on a small matrix
+  if (forced_shift >= 0) p.item_shift = forced_shift;
   const int64_t n_items = (p.M + (1 << p.item_shift) - 1) >> p.item_shift;
   TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
   const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);

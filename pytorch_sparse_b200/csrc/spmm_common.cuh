@@ -2,6 +2,8 @@
 // work-queue records, kernel parameters, the per-warp cp.async index ring and the 16-byte vector math.
 #pragma once
 
+#include <cstdlib>
+
 #include "common.cuh"
 
 namespace tsb {
@@ -355,5 +357,16 @@ struct GridCache {
     return g;
   }
 };
+
+// TSB200_SPMM_ITEM_SHIFT = 0..5, read on every call, fixes the work item of the SpMM forward and SDDMM row kernels at
+// 2^s rows: a test knob, so that small matrices can run every item size. Unset or out of range: -1 (the launch's own
+// choice stands).
+static inline int item_shift_override() {
+  const char* ev = getenv("TSB200_SPMM_ITEM_SHIFT");
+  if (!ev) return -1;
+  char* end = nullptr;
+  const long v = strtol(ev, &end, 10);
+  return (end != ev && *end == '\0' && v >= 0 && v <= 5) ? (int)v : -1;
+}
 
 }  // namespace tsb

@@ -1186,6 +1186,8 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
   int64_t want = p.M * p.B / ((int64_t)grid_main * kWarpsPerCta * 2);
   p.item_shift = 0;
   while (p.item_shift < 5 && ((int64_t)2 << p.item_shift) <= want) p.item_shift++;
+  const int forced_shift = item_shift_override();  // tests: every item size on a small matrix
+  if (forced_shift >= 0) p.item_shift = forced_shift;
   const int64_t n_items = ((p.M + (1 << p.item_shift) - 1) >> p.item_shift) * p.B;
   for (int k0 = 0; k0 < p.K; k0 += kcols) {
     p.k0 = k0;

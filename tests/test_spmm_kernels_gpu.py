@@ -151,11 +151,12 @@ def sub_csr(rowptr, col, rows):
     return sp, col[idx], idx
 
 
-def plan_budget_rows(rowptr):
-    """Rows the plan defers for the 1024-nnz budget of their 32-row group (not for their length)."""
+def plan_budget_rows(rowptr, group=32):
+    """Rows deferred for the 1024-nnz budget of their `group`-row work item (not for their length): the plan's rule
+    with the default 32, an unplanned call's with the size of its items."""
     deg = rowptr[1:] - rowptr[:-1]
     M = deg.numel()
-    d = torch.cat([deg, deg.new_zeros((-M) % 32)]).view(-1, 32)
+    d = torch.cat([deg, deg.new_zeros((-M) % group)]).view(-1, group)
     cum = torch.where(d > 256, 0, d).cumsum(1)
     return ((d > 0) & (d <= 256) & (cum > 1024)).view(-1)[:M]
 
@@ -351,7 +352,7 @@ def test_dispatch_table_matches_library(small, dtype, K):
     plan = ops.spmm_plan(rowptr, col.numel())
     for planned in (False, True):
         names = launched_kernels(lambda: call_planned(plan, rowptr, col, None, mat, "sum") if planned
-                          else call_fw(rowptr, col, None, mat, "sum"))
+                          else call_fw(rowptr, col, None, mat, "sum"), r"spmm_(gpr|vec)_kernel<")
         if fam.startswith("gpr"):
             got = [int(m.group(1)) for n in names for m in [re.search(r"spmm_gpr_kernel<[^,]+, \d+, (\d+), (\d+), (\d+)", n)]
                    if m and m.group(2) == "4" and m.group(3) == "5"]

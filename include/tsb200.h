@@ -237,6 +237,30 @@ TSB200_API int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
                          size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * SDDMM over two FP8 (e4m3) operands with per-tensor or per-row scales: edge scores <a[row_e], b[col_e]> of quantised
+ * embeddings (no counterpart in the reference).  B = 1.
+ *   For every entry e of the CSR structure (rowptr, col), row r, column c:
+ *     d_e = sum_k a8[r,k] * b8[c,k]   (each product exact in fp32, the sum in fp32 in the kernel's lane order,
+ *                                      starting from +0)
+ *     s_e = fl32(a_scale[r * a_scale_stride] * b_scale[c * b_scale_stride])   (strides 0: one scale per operand)
+ *     out[e] = round_out(fl32(s_e * d_e))   (round to nearest even; no FMA contraction)
+ *   a8 e4m3[M, K], b8 e4m3[N, K], both contiguous and 16-byte aligned, K % 16 == 0 and K <= 2048; a_scale / b_scale
+ *   f32, 4-byte aligned; out out_dtype[E] in CSR order, out_dtype in {F32, F16, BF16}. NaN in either operand or scale
+ *   propagates; +-0 follows IEEE. The work decomposition is tsb200_spmm_value_bw's row-wise kernel: the a8 row is
+ *   loaded once per CSR row, b8 rows are gathered; rows over 256 entries go through the device-side segment queue.
+ *   workspace: tsb200_sddmm_fp8_workspace_bytes(M, K, E) bytes, 256 B aligned (0 when E == 0 or K == 0).
+ *   E == 0: nothing is launched. K == 0: out = +0 (a memset). TSB200_ERR_INVALID_ARG for a negative extent, a scale
+ *   stride other than 0 / 1, a NULL pointer, a missing or misaligned workspace; TSB200_ERR_UNSUPPORTED for another
+ *   out_dtype, K % 16 != 0, K > 2048, E >= 2^31 - 64, M or N >= 2^32, or a misaligned pointer (a8 / b8 16 B, col 8 B,
+ *   scales 4 B, out its element size); TSB200_ERR_WORKSPACE for a short workspace.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API size_t tsb200_sddmm_fp8_workspace_bytes(int64_t M, int64_t K, int64_t E);
+TSB200_API int tsb200_sddmm_fp8(const int64_t* rowptr, const int64_t* col, const void* a8, const float* a_scale,
+                                int64_t a_scale_stride, const void* b8, const float* b_scale, int64_t b_scale_stride,
+                                void* out, int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Fused min/max backward.  Replaces the ATen chain in SPMMMin/SPMMMax::backward
  *   (csrc/spmm.cpp:204-242, 264-302): for every (b,m,k) with a = arg_out[b,m,k] != E,
  *     grad_value[a]           += mat[b,col[a],k] * grad_out[b,m,k]      (if grad_value != NULL)

@@ -7,6 +7,7 @@
 //    row/col coalesced, LPR lanes x 16 B cover one dense row, the 32/LPR lane groups work on
 //    different nnz, results are gathered back to one lane per nnz for a coalesced store.
 //    grad[row[e]] is re-read per nnz but consecutive nnz share the row => L1/L2 hits.
+//  * tsb200_sddmm_fp8: the row-wise SDDMM kernels over two e4m3 operands with per-row or per-tensor scales.
 //  * tsb200_spmm_minmax_bw: fused replacement of the 8-op ATen chain of SPMMMin/SPMMMax::backward
 //    (csrc/spmm.cpp:204-242, 264-302): one pass over arg_out, atomics into zero-filled fp32/fp64
 //    accumulators.
@@ -42,6 +43,22 @@ template <> struct Vec16<__nv_bfloat16, 8> {
 };
 template <> struct Vec16<__half, 8> {
   static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) { return dot16<__half>(a, b); }
+};
+// e4m3 (tsb200_sddmm_fp8): 16 elements per vector, widened exactly (Vec<__nv_fp8_e4m3>::unpack); the product of two
+// e4m3 values is exact in fp32, so as above FFMA rounds once per term, even and odd elements accumulated separately.
+template <> struct Vec16<__nv_fp8_e4m3, 16> {
+  static __device__ __forceinline__ float dot(const uint4& a, const uint4& b) {
+    float x[16], y[16];
+    Vec<__nv_fp8_e4m3>::unpack(a, x);
+    Vec<__nv_fp8_e4m3>::unpack(b, y);
+    float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      s0 = fmaf(x[2 * i], y[2 * i], s0);
+      s1 = fmaf(x[2 * i + 1], y[2 * i + 1], s1);
+    }
+    return s0 + s1;
+  }
 };
 
 // Reduce U per-lane partial sums over the W*2 lanes of a lane group with a halving butterfly:
@@ -157,8 +174,12 @@ value_bw_vec_kernel(const int64_t* __restrict__ row, const int64_t* __restrict__
 // grad vector is loaded ONCE into registers (16 B per lane and chunk), so only the dense-operand rows are
 // gathered (half the L1/L2 traffic of the nnz-parallel kernel); every nnz's dot product is reduced over the
 // LPR lanes with the halving butterfly and the chunk's results leave with one coalesced store.
-template <typename T, int LPR, int CH, int U> struct SddmmEngine {
-  static constexpr int VEC = 16 / sizeof(T);
+// T = output type, X = type of both dense operands: T itself, or __nv_fp8_e4m3 (tsb200_sddmm_fp8). For e4m3 a vector
+// is 16 columns, `scale` is the row operand's scale of the row, and the gathered row's scale bscale[c * bstride] is
+// loaded next to its column word; after the reduction out = round_T(fl32(fl32(scale * bscale[c]) * dot)).
+template <typename T, int LPR, int CH, int U, typename X = T> struct SddmmEngine {
+  static constexpr bool Q8 = !std::is_same<X, T>::value;
+  static constexpr int VEC = 16 / sizeof(X);
   static constexpr int G = 32 / LPR;
   uint4 gq[CH];
 
@@ -171,7 +192,8 @@ template <typename T, int LPR, int CH, int U> struct SddmmEngine {
   // ring-relative nnz [s, e) of one row -> out[absolute nnz]
   __device__ __forceinline__ void run(IndexRing<T>& ring, int s, int e, const char* __restrict__ matb,
                                       uint32_t row_bytes, const bool (&col_ok)[CH], int lane, int g, int li,
-                                      uint64_t pol, T* __restrict__ out, float scale) {
+                                      uint64_t pol, T* __restrict__ out, float scale,
+                                      const float* __restrict__ bscale = nullptr, uint32_t bstride = 0) {
     for (int j0 = s; j0 < e; j0 += U * G) {
       const int jend = min(e, j0 + U * G);
       ring.ensure(j0, jend, lane);
@@ -181,6 +203,7 @@ template <typename T, int LPR, int CH, int U> struct SddmmEngine {
       const int jrel = jend - j0 - g;
       uint4 d[U][CH];
       float part[U];
+      float sc[U];  // Q8 only: scale of each step's gathered row
       // Branch-free chunk (the kernel is issue-bound, and branches around the inline-asm gathers cost issue slots):
       // the gathers are predicated inside the asm into zeroed
       // registers and the dot products run unconditionally (an inactive slot contributes 0). The ring slot is read
@@ -196,28 +219,43 @@ template <typename T, int LPR, int CH, int U> struct SddmmEngine {
           d[u][ch] = make_uint4(0, 0, 0, 0);
           ldg128_hint_pred(d[u][ch], src + ch * (LPR * 16), pol, act && col_ok[ch]);
         }
+        if constexpr (Q8) sc[u] = act ? __ldg(bscale + (size_t)c * bstride) : 0.f;
       }
 #pragma unroll
       for (int u = 0; u < U; u++) {
         float sdot = 0.f;
 #pragma unroll
-        for (int ch = 0; ch < CH; ch++) sdot += Vec16<T, VEC>::dot(d[u][ch], gq[ch]);
+        for (int ch = 0; ch < CH; ch++) sdot += Vec16<X, VEC>::dot(d[u][ch], gq[ch]);
         part[u] = sdot;
       }
       // lane li of group g gets the total of step li / (LPR/U); nnz t = u*G + g of the chunk goes to lane t
-      const float tot = multi_reduce<U, LPR / 2>(part, li);
+      float tot = multi_reduce<U, LPR / 2>(part, li);
+      if constexpr (Q8) {  // the scale product, on the lane that holds the step's total
+        const int ul = li / (LPR / U);
+        float sb = sc[0];
+#pragma unroll
+        for (int u = 1; u < U; u++)
+          if (ul == u) sb = sc[u];
+        tot = __fmul_rn(__fmul_rn(scale, sb), tot);
+      }
       const bool mine = lane < jend - j0;
       const int src_lane = mine ? (lane % G) * LPR + (lane / G) * (LPR / U) : 0;
       const float got = __shfl_sync(0xffffffffu, tot, src_lane);
-      if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got * scale);
+      if constexpr (Q8) {
+        if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got);
+      } else {
+        if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got * scale);
+      }
     }
   }
 };
 
-template <typename T, int LPR, int CH, int U, int MINB>
+// X = e4m3: gscale[row * gstride] is the row operand's scale, p.scale[col * p.scale_stride] the gathered row's
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
-sddmm_vec_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__ out) {
-  using Eng = SddmmEngine<T, LPR, CH, U>;
+sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__ out, const float* __restrict__ gscale,
+                 uint32_t gstride) {
+  using Eng = SddmmEngine<T, LPR, CH, U, X>;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -235,7 +273,7 @@ sddmm_vec_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = (ch * LPR + li) * VEC < p.K;
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
   const char* matb = (const char*)p.mat + (int64_t)li * 16;
   asm volatile("" : "+l"(matb));
 
@@ -288,17 +326,23 @@ sddmm_vec_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__
       if (e == s) continue;
       Eng eng;
       eng.load_grad((const char*)grad + (r0 + rl) * (int64_t)row_bytes, col_ok, li);
-      const float scale = p.mean ? 1.f / (float)(e - s) : 1.f;
-      eng.run(ring, s, e, matb, row_bytes, col_ok, lane, g, li, pol, out, scale);
+      if constexpr (Eng::Q8) {
+        const float scale = __ldg(gscale + (r0 + rl) * gstride);
+        eng.run(ring, s, e, matb, row_bytes, col_ok, lane, g, li, pol, out, scale, p.scale, p.scale_stride);
+      } else {
+        const float scale = p.mean ? 1.f / (float)(e - s) : 1.f;
+        eng.run(ring, s, e, matb, row_bytes, col_ok, lane, g, li, pol, out, scale);
+      }
     }
     item = __shfl_sync(0xffffffffu, next_item, 0);
   }
 }
 
-template <typename T, int LPR, int CH, int U, int MINB>
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
-sddmm_seg_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__ out) {
-  using Eng = SddmmEngine<T, LPR, CH, U>;
+sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__ out, const float* __restrict__ gscale,
+                 uint32_t gstride) {
+  using Eng = SddmmEngine<T, LPR, CH, U, X>;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -314,7 +358,7 @@ sddmm_seg_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = (ch * LPR + li) * VEC < p.K;
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
   const char* matb = (const char*)p.mat + (int64_t)li * 16;
   asm volatile("" : "+l"(matb));
 
@@ -326,20 +370,26 @@ sddmm_seg_kernel(const SpmmParams p, const T* __restrict__ grad, T* __restrict__
     ring.reset(base, S.end);
     Eng eng;
     eng.load_grad((const char*)grad + S.row_b * (int64_t)row_bytes, col_ok, li);
-    float scale = 1.f;
-    if (p.mean) {
-      const int64_t cnt = __ldg(p.rowptr + S.row_b + 1) - __ldg(p.rowptr + S.row_b);
-      scale = 1.f / (float)(cnt > 0 ? cnt : 1);
+    if constexpr (Eng::Q8) {
+      eng.run(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, li, pol, out,
+              __ldg(gscale + S.row_b * gstride), p.scale, p.scale_stride);
+    } else {
+      float scale = 1.f;
+      if (p.mean) {
+        const int64_t cnt = __ldg(p.rowptr + S.row_b + 1) - __ldg(p.rowptr + S.row_b);
+        scale = 1.f / (float)(cnt > 0 ? cnt : 1);
+      }
+      eng.run(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, li, pol, out, scale);
     }
-    eng.run(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, li, pol, out, scale);
     __syncwarp();
   }
 }
 
-template <typename T, int LPR, int CH, int U, int MINB>
-static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t st) {
-  auto* kmain = sddmm_vec_kernel<T, LPR, CH, U, MINB>;
-  auto* kseg = sddmm_seg_kernel<T, LPR, CH, U, MINB>;
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
+static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t st, const float* gscale = nullptr,
+                        uint32_t gstride = 0) {
+  auto* kmain = sddmm_vec_kernel<T, LPR, CH, U, MINB, X>;
+  auto* kseg = sddmm_seg_kernel<T, LPR, CH, U, MINB, X>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
@@ -351,9 +401,9 @@ static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t 
   const int64_t n_items = (p.M + (1 << p.item_shift) - 1) >> p.item_shift;
   TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
   const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);
-  kmain<<<gm, kWarpsPerCta * 32, 0, st>>>(p, (const T*)grad, (T*)out);
+  kmain<<<gm, kWarpsPerCta * 32, 0, st>>>(p, (const X*)grad, (T*)out, gscale, gstride);
   TSB_LAUNCH_CHECK();
-  kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p, (const T*)grad, (T*)out);
+  kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p, (const X*)grad, (T*)out, gscale, gstride);
   TSB_LAUNCH_CHECK();
   return 0;
 }
@@ -366,6 +416,20 @@ template <typename T> static int dispatch_sddmm(const SpmmParams& p, const void*
   if (vecs <= 16) return launch_sddmm<T, 16, 1, 4, 5>(p, grad, out, st);
   if (vecs <= 32) return launch_sddmm<T, 32, 1, 4, 4>(p, grad, out, st);
   return launch_sddmm<T, 32, 2, 4, 3>(p, grad, out, st);  // up to 64 vectors
+}
+
+// e4m3 operands, output type T: a vector is 16 columns, so a K-column row is K / 16 vectors (K <= 2048)
+template <typename T>
+static int dispatch_sddmm_fp8(const SpmmParams& p, const void* a8, void* out, cudaStream_t st, const float* a_scale,
+                              uint32_t a_stride) {
+  using X = __nv_fp8_e4m3;
+  const int64_t vecs = p.K / 16;
+  if (vecs <= 4) return launch_sddmm<T, 4, 1, 4, 4, X>(p, a8, out, st, a_scale, a_stride);
+  if (vecs <= 8) return launch_sddmm<T, 8, 1, 4, 4, X>(p, a8, out, st, a_scale, a_stride);
+  if (vecs <= 16) return launch_sddmm<T, 16, 1, 4, 4, X>(p, a8, out, st, a_scale, a_stride);
+  if (vecs <= 32) return launch_sddmm<T, 32, 1, 4, 4, X>(p, a8, out, st, a_scale, a_stride);
+  if (vecs <= 64) return launch_sddmm<T, 32, 2, 4, 3, X>(p, a8, out, st, a_scale, a_stride);
+  return launch_sddmm<T, 32, 4, 2, 2, X>(p, a8, out, st, a_scale, a_stride);  // up to 128 vectors
 }
 
 // generic: warp per nnz, lanes stride over k (any dtype / alignment).
@@ -530,6 +594,63 @@ extern "C" int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
     TSB_LAUNCH_CHECK();
     return 0;
   });
+}
+
+// ---- SDDMM over two e4m3 operands with per-tensor or per-row scales ------------------------------------------------
+// The row-wise kernels with X = __nv_fp8_e4m3 and T = out_dtype: `mat` is b8 [N, K] (gathered, p.scale = b_scale) and
+// `grad` is a8 [M, K] (one row in registers per CSR row, its scale read once per row).
+extern "C" size_t tsb200_sddmm_fp8_workspace_bytes(int64_t M, int64_t K, int64_t E) {
+  (void)M;
+  if (K <= 0 || E <= 0) return 0;
+  return ws_layout(1, K, E, false, false).total;
+}
+
+extern "C" int tsb200_sddmm_fp8(const int64_t* rowptr, const int64_t* col, const void* a8, const float* a_scale,
+                                int64_t a_scale_stride, const void* b8, const float* b_scale, int64_t b_scale_stride,
+                                void* out, int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || K < 0 || E < 0) return TSB200_ERR_INVALID_ARG;
+  if ((a_scale_stride != 0 && a_scale_stride != 1) || (b_scale_stride != 0 && b_scale_stride != 1))
+    return TSB200_ERR_INVALID_ARG;
+  if (out_dtype != TSB200_F32 && out_dtype != TSB200_F16 && out_dtype != TSB200_BF16) return TSB200_ERR_UNSUPPORTED;
+  if (K % 16 != 0 || K > 2048) return TSB200_ERR_UNSUPPORTED;
+  if (E == 0) return 0;
+  if (!out) return TSB200_ERR_INVALID_ARG;
+  const size_t es = dtype_size(out_dtype);
+  if ((uintptr_t)out % es) return TSB200_ERR_UNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (K == 0) {  // every dot product is empty: +0
+    TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)E * es, st));
+    return 0;
+  }
+  if (!rowptr || !col || !a8 || !a_scale || !b8 || !b_scale) return TSB200_ERR_INVALID_ARG;
+  if (E >= ((int64_t)1 << 31) - 64 || N >= ((int64_t)1 << 32) || M >= ((int64_t)1 << 32)) return TSB200_ERR_UNSUPPORTED;
+  if (((uintptr_t)a8 & 15) || ((uintptr_t)b8 & 15) || ((uintptr_t)col & 7) || ((uintptr_t)a_scale & 3) ||
+      ((uintptr_t)b_scale & 3))
+    return TSB200_ERR_UNSUPPORTED;
+  if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
+  const WsLayout L = ws_layout(1, K, E, false, false);
+  if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+  char* ws = (char*)workspace;
+  SpmmParams p;
+  p.rowptr = rowptr; p.col = col; p.value = nullptr; p.mat = b8; p.out = nullptr; p.arg_out = nullptr;
+  p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
+  p.partial = nullptr; p.acc_mode = 0;
+  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
+  p.counters = (unsigned int*)(ws + L.counters);
+  p.segs = (Segment*)(ws + L.segs);
+  p.longs = (LongRow*)(ws + L.longs);
+  p.part_val = nullptr; p.part_arg = nullptr;
+  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+  p.scale = b_scale; p.scale_stride = (uint32_t)b_scale_stride;
+  p.out_scale = nullptr; p.res8 = nullptr; p.res_scale = nullptr; p.res_stride = 0;
+  const uint32_t as = (uint32_t)a_scale_stride;
+  switch (out_dtype) {
+    case TSB200_F32: return dispatch_sddmm_fp8<float>(p, a8, out, st, a_scale, as);
+    case TSB200_F16: return dispatch_sddmm_fp8<__half>(p, a8, out, st, a_scale, as);
+    case TSB200_BF16: return dispatch_sddmm_fp8<__nv_bfloat16>(p, a8, out, st, a_scale, as);
+  }
+  return TSB200_ERR_UNSUPPORTED;
 }
 
 extern "C" int tsb200_spmm_minmax_bw(const int64_t* col, const void* value, const void* mat,

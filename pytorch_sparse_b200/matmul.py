@@ -143,6 +143,43 @@ def quantize_fp8(x: Tensor, per_row: bool = True) -> Tuple[Tensor, Tensor]:
     return x8, scale
 
 
+def sddmm(src: SparseTensor, a: Tensor, b: Tensor) -> Tensor:
+    """Edge scores `out[e] = <a[row_e], b[col_e]>` for every stored entry of `src` (M x N), in CSR order, without an
+    E x K temporary: `a` [M, K] and `b` [N, K] share a floating dtype (bf16, f16, f32, f64), accumulated in fp32
+    (fp64 for fp64) and rounded once. `src`'s values are ignored: only its structure is used. Differentiable in `a` and
+    `b`; the gradients are SpMMs with the incoming gradient as values, on the CSR view for `a` and on the cached CSC
+    view for `b`. To score arbitrary pairs (i, j), build `SparseTensor(row=i, col=j, value=arange)` and scatter the
+    scores back through its permuted values (see README)."""
+    rowptr, col, _ = src.csr()
+    st = src.storage
+    M, N = src.sparse_sizes()
+    if a.dim() == 2 and b.dim() == 2 and (a.size(0) != M or b.size(0) != N):
+        raise RuntimeError("sddmm: a must have " + str(M) + " rows and b " + str(N) + " rows (the sparse sizes), got "
+                           + str(a.size(0)) + " and " + str(b.size(0)))
+    row = st.row()
+    colptr, csr2csc = st._colptr, st._csr2csc
+    row_csc: Optional[Tensor] = None
+    if b.requires_grad:     # grad_b = A(g)^T @ a runs on the CSC view
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.sddmm(row, rowptr, col, colptr, csr2csc, row_csc, a, b)
+
+
+def sddmm_fp8(src: SparseTensor, a8: Tensor, a_scale: Tensor, b8: Tensor, b_scale: Tensor,
+              out_dtype: torch.dtype = torch.float32) -> Tensor:
+    """`sddmm` over two FP8 (e4m3) operands with float32 scales of shape [] or [rows] (see `quantize_fp8`):
+    `out[e] = round_out(fl32(a_scale[r] * b_scale[c]) * sum_k a8[r, k] * b8[c, k])`, the sum in fp32 (every e4m3
+    product is exact). `a8` [M, K] and `b8` [N, K] contiguous and 16-byte aligned, K % 16 == 0 and K <= 2048 (a
+    ValueError otherwise); out_dtype bf16, f16 or f32. `src`'s values are ignored. Forward only: a scale that requires
+    grad is refused while grad mode is on."""
+    rowptr, col, _ = src.csr()
+    N = src.sparse_size(1)
+    if b8.dim() == 2 and b8.size(0) != N:
+        raise RuntimeError("sddmm_fp8: b8 must have " + str(N) + " rows (the sparse sizes), got " + str(b8.size(0)))
+    return torch.ops.tsb200.sddmm_fp8(rowptr, col, a8, a_scale, b8, b_scale, out_dtype)
+
+
 def spspmm_sum(src: SparseTensor, other: SparseTensor) -> SparseTensor:
     M, Kd = src.sparse_sizes()
     Kb, N = other.sparse_sizes()
@@ -201,6 +238,9 @@ SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bf
     residual_scale=None: spmm_fp8(self, x8, scale, reduce, out_dtype, residual, residual_scale)
 SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum", residual=None, residual_scale=None: spmm_fp8_quant(
     self, x8, scale, reduce, residual, residual_scale)
+SparseTensor.sddmm = lambda self, a, b: sddmm(self, a, b)
+SparseTensor.sddmm_fp8 = lambda self, a8, a_scale, b8, b_scale, out_dtype=torch.float32: sddmm_fp8(
+    self, a8, a_scale, b8, b_scale, out_dtype)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)
 SparseTensor.__matmul__ = lambda self, other: matmul(self, other, "sum")

@@ -1063,6 +1063,127 @@ def spmm_max(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor) 
     return SPMMMax.apply(rowptr, col, value, mat)
 
 
+# --------------------------------------------------------------------------------------------------
+# SDDMM: per-entry dot products of two dense operands
+# --------------------------------------------------------------------------------------------------
+def _sddmm_check(rowptr: Tensor, col: Tensor, a: Tensor, b: Tensor, colptr: Optional[Tensor]) -> None:
+    for t, n in ((rowptr, "rowptr"), (col, "col"), (a, "a"), (b, "b")):
+        _check_cuda(t, n)
+    for t, n in ((a, "a"), (b, "b")):
+        if t.dim() != 2:
+            raise RuntimeError(f"sddmm: {n} must be 2-D, got {t.dim()}-D")
+    if not a.dtype.is_floating_point or a.dtype not in _DTYPES:
+        raise RuntimeError(f'"sddmm" not implemented for \'{a.dtype}\'')
+    if b.dtype != a.dtype:
+        raise RuntimeError(f"sddmm: a and b must have the same dtype, got {a.dtype} and {b.dtype}")
+    M = rowptr.numel() - 1
+    if a.size(0) != M or a.size(1) != b.size(1):
+        raise RuntimeError(f"sddmm: a must be [M, K] = [{M}, {b.size(1)}] for b of shape {list(b.shape)}, "
+                           f"got {list(a.shape)}")
+    if colptr is not None and colptr.numel() - 1 != b.size(0):
+        raise RuntimeError(f"sddmm: b must have {colptr.numel() - 1} rows (the matrix's columns), got {b.size(0)}")
+
+
+class SDDMM(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, row, rowptr, col, colptr, csr2csc, row_csc, a, b):
+        need_a, need_b = ctx.needs_input_grad[6], ctx.needs_input_grad[7]
+        if need_b:
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+        # the SpMM value gradient with grad := a, mat := b (tsb200_spmm_value_bw, reduce = sum)
+        out = spmm_value_bw(row, rowptr, col, b, a, "sum")
+        ctx.save_for_backward(row if need_b else None, rowptr if need_a else None, col if need_a else None,
+                              colptr if need_b else None, csr2csc if need_b else None,
+                              row_csc if need_b else None, a if need_b else None, b if need_a else None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row, rowptr, col, colptr, csr2csc, row_csc, a, b = ctx.saved_tensors
+        grad_a = grad_b = None
+        if ctx.needs_input_grad[6]:     # grad_a = A(g) @ b on the CSR view
+            grad_a, _ = spmm_fw(rowptr, col, grad_out, b, "sum")
+        if ctx.needs_input_grad[7]:     # grad_b = A(g)^T @ a on the CSC view
+            if row_csc is None:
+                row_csc = row.index_select(0, csr2csc)
+            grad_b, _ = spmm_fw(colptr, row_csc, grad_out.index_select(0, csr2csc), a, "sum")
+        return None, None, None, None, None, None, grad_a, grad_b
+
+
+def sddmm(row: Tensor, rowptr: Tensor, col: Tensor, colptr: Optional[Tensor], csr2csc: Optional[Tensor],
+          row_csc: Optional[Tensor], a: Tensor, b: Tensor) -> Tensor:
+    """`out[e] = <a[row[e]], b[col[e]]>` for every entry of the CSR structure (rowptr, col), in CSR order, with `row`
+    its COO row. `a` [M, K] and `b` [N, K] share a floating dtype; fp32 accumulation (fp64 for fp64), one rounding to
+    the dtype. Differentiable in `a` (an SpMM on the CSR view) and `b` (an SpMM on the CSC view, which needs `colptr`,
+    `csr2csc` and optionally the cached `row_csc = row[csr2csc]`)."""
+    _sddmm_check(rowptr, col, a, b, colptr)
+    return SDDMM.apply(row, rowptr, col, colptr, csr2csc, row_csc, a, b)
+
+
+FP8_SDDMM_MAX_K = 2048
+
+
+def _fp8_scale(what: str, name: str, scale: Tensor, rows: int) -> int:
+    if scale.dtype != torch.float32:
+        raise RuntimeError(f"{what}: {name} must be float32, got {scale.dtype}")
+    if scale.dim() == 0:
+        return 0
+    if scale.dim() == 1 and scale.size(0) == rows:
+        return 1
+    raise RuntimeError(f"{what}: {name} must have shape [] or [{rows}], got {list(scale.shape)}")
+
+
+def sddmm_fp8(rowptr: Tensor, col: Tensor, a8: Tensor, a_scale: Tensor, b8: Tensor, b_scale: Tensor,
+              out_dtype: torch.dtype = torch.float32) -> Tensor:
+    """`sddmm_fp8(rowptr, col, a8, a_scale, b8, b_scale, out_dtype) -> out[E]` (tsb200_sddmm_fp8): per entry e (row r,
+    column c) the dot product of two e4m3 rows, out[e] = round_out(fl32(fl32(a_scale[r] * b_scale[c]) * d_e)) with
+    d_e = sum_k a8[r, k] * b8[c, k] accumulated in fp32 (every product exact). `a8` [M, K] and `b8` [N, K] are
+    contiguous, 16-byte aligned e4m3 (as `quantize_fp8` makes them), K % 16 == 0 and K <= 2048; scales are float32 of
+    shape [] or [rows]; out_dtype bf16, f16 or f32. Forward only."""
+    what = "sddmm_fp8"
+    for t, n in ((rowptr, "rowptr"), (col, "col"), (a8, "a8"), (a_scale, "a_scale"), (b8, "b8"), (b_scale, "b_scale")):
+        _check_cuda(t, n)
+    if torch.is_grad_enabled() and (a_scale.requires_grad or b_scale.requires_grad):
+        raise RuntimeError(f"{what} is forward only: a_scale and b_scale must not require grad "
+                           "(call it under torch.no_grad() or detach them)")
+    for t, n in ((a8, "a8"), (b8, "b8")):
+        if t.dtype != torch.float8_e4m3fn:
+            raise RuntimeError(f"{what}: {n} must be torch.float8_e4m3fn, got {t.dtype}")
+        if t.dim() != 2:
+            raise RuntimeError(f"{what}: {n} must be 2-D, got {t.dim()}-D")
+    M = rowptr.numel() - 1
+    K = b8.size(1)
+    if a8.size(0) != M or a8.size(1) != K:
+        raise RuntimeError(f"{what}: a8 must be [M, K] = [{M}, {K}] for b8 of shape {list(b8.shape)}, "
+                           f"got {list(a8.shape)}")
+    if K % 16 != 0:
+        raise ValueError(f"{what}: the number of columns K = {K} must be a multiple of 16")
+    if K > FP8_SDDMM_MAX_K:
+        raise ValueError(f"{what}: the number of columns K = {K} must be at most {FP8_SDDMM_MAX_K}")
+    for t, n in ((a8, "a8"), (b8, "b8")):
+        if not t.is_contiguous() or t.data_ptr() % 16 != 0:
+            raise RuntimeError(f"{what}: {n} must be contiguous and 16-byte aligned")
+    if out_dtype not in _FP8_OUT:
+        raise RuntimeError(f"{what}: out_dtype must be torch.bfloat16, torch.float16 or torch.float32, got {out_dtype}")
+    sa = _fp8_scale(what, "a_scale", a_scale, M)
+    sb = _fp8_scale(what, "b_scale", b_scale, b8.size(0))
+    _check_input(rowptr.dim() == 1 and col.dim() == 1)
+    rowptr, col = _i64(rowptr, "rowptr"), _i64(col, "col")
+    a_scale, b_scale = a_scale.contiguous(), b_scale.contiguous()
+    E, N = col.numel(), b8.size(0)
+    dev = b8.device
+    if E == 0 or M == 0 or K == 0:     # nothing to launch; an empty dot product is +0
+        return torch.zeros(E, dtype=out_dtype, device=dev)
+    out = torch.empty(E, dtype=out_dtype, device=dev)
+    with _on_device(dev):
+        nws = lib.tsb200_sddmm_fp8_workspace_bytes(M, K, E)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_sddmm_fp8(_p(rowptr), _p(col), _p(a8), _p(a_scale), sa, _p(b8), _p(b_scale), sb, _p(out),
+                                   M, N, K, E, _FP8_OUT[out_dtype], _p(ws), nws, _stream(dev)), "tsb200_sddmm_fp8")
+    return out
+
+
 def cuda_version() -> int:
     """CUDA toolkit version of the native library in CUDA_VERSION encoding, like
     torch.ops.torch_sparse.cuda_version() (csrc/version.cpp:27-41)."""

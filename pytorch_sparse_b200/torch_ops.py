@@ -3,7 +3,7 @@
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
     torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant,
-                      quantize_fp8}  (own additions)
+                      quantize_fp8, sddmm, sddmm_fp8}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -50,6 +50,11 @@ _EXTRA_SCHEMAS = {
     "spmm_fp8_quant": "(Tensor rowptr, Tensor col, Tensor? value, Tensor x8, Tensor scale, str reduce, "
                       "Tensor? residual=None, Tensor? residual_scale=None) -> (Tensor, Tensor, Tensor?)",
     "quantize_fp8": "(Tensor x, bool per_row) -> (Tensor, Tensor)",
+    # per-entry dot products <a[row_e], b[col_e]>; colptr / csr2csc / row_csc (the CSC view) only for a gradient to b
+    "sddmm": "(Tensor row, Tensor rowptr, Tensor col, Tensor? colptr, Tensor? csr2csc, Tensor? row_csc, Tensor a, "
+             "Tensor b) -> Tensor",
+    "sddmm_fp8": "(Tensor rowptr, Tensor col, Tensor a8, Tensor a_scale, Tensor b8, Tensor b_scale, "
+                 "ScalarType out_dtype) -> Tensor",
 }
 
 
@@ -69,6 +74,7 @@ _EXTRA_IMPLS = {
     "spmm_fp8_quant": lambda rowptr, col, value, x8, scale, reduce, residual=None, residual_scale=None:
         ops.spmm_fw_fp8_quant(rowptr, col, value, x8, scale, reduce, residual=residual, residual_scale=residual_scale),
     "quantize_fp8": ops.quantize_fp8,
+    "sddmm": ops.sddmm, "sddmm_fp8": ops.sddmm_fp8,
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -294,14 +294,7 @@ sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
     const int64_t base = a0 & ~(int64_t)31;
     const int s_rel = (int)(rp0 - base), e_rel = (int)(rp1 - base);
     const int deg = e_rel - s_rel;
-    const bool is_long = deg > kLongT;
-    int cum = is_long ? 0 : deg;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, cum, off);
-      if (lane >= off) cum += t;
-    }
-    const bool defer = (deg > 0) && (is_long || cum > kItemCap);
+    const bool defer = defer_row(deg, lane);
     const unsigned defer_mask = __ballot_sync(0xffffffffu, defer);
     if (defer) {
       const int nseg = (deg + kSeg - 1) / kSeg;
@@ -393,11 +386,7 @@ static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t 
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
-  int64_t want = p.M / ((int64_t)grid_main * kWarpsPerCta * 2);
-  p.item_shift = 0;
-  while (p.item_shift < 5 && ((int64_t)2 << p.item_shift) <= want) p.item_shift++;
-  const int forced_shift = item_shift_override();  // tests: every item size on a small matrix
-  if (forced_shift >= 0) p.item_shift = forced_shift;
+  p.item_shift = item_shift_for(p.M, grid_main);
   const int64_t n_items = (p.M + (1 << p.item_shift) - 1) >> p.item_shift;
   TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
   const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);
@@ -558,17 +547,9 @@ extern "C" int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
       !((uintptr_t)workspace & 255)) {
     const WsLayout L = ws_layout(1, K, E, false, false);
     if (workspace_bytes >= L.total) {
-      char* ws = (char*)workspace;
-      SpmmParams p;
-      p.rowptr = rowptr; p.col = col; p.value = nullptr; p.mat = mat; p.out = nullptr; p.arg_out = nullptr;
-      p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = mean ? 1 : 0; p.item_shift = 5;
-      p.partial = nullptr; p.acc_mode = 0;
-      p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-      p.counters = (unsigned int*)(ws + L.counters);
-      p.segs = (Segment*)(ws + L.segs);
-      p.longs = (LongRow*)(ws + L.longs);
-      p.part_val = nullptr; p.part_arg = nullptr;
-      p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+      SpmmParams p{rowptr, col, nullptr, mat, nullptr, nullptr, 1, M, N, K, E};
+      p.mean = mean ? 1 : 0;
+      bind_ws(p, (char*)workspace, L, false);
       switch (dtype) {
         case TSB200_F32: return dispatch_sddmm<float>(p, grad, out, st);
         case TSB200_F16: return dispatch_sddmm<__half>(p, grad, out, st);
@@ -631,19 +612,9 @@ extern "C" int tsb200_sddmm_fp8(const int64_t* rowptr, const int64_t* col, const
   if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
   const WsLayout L = ws_layout(1, K, E, false, false);
   if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-  char* ws = (char*)workspace;
-  SpmmParams p;
-  p.rowptr = rowptr; p.col = col; p.value = nullptr; p.mat = b8; p.out = nullptr; p.arg_out = nullptr;
-  p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
-  p.partial = nullptr; p.acc_mode = 0;
-  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-  p.counters = (unsigned int*)(ws + L.counters);
-  p.segs = (Segment*)(ws + L.segs);
-  p.longs = (LongRow*)(ws + L.longs);
-  p.part_val = nullptr; p.part_arg = nullptr;
-  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+  SpmmParams p{rowptr, col, nullptr, b8, nullptr, nullptr, 1, M, N, K, E};
+  bind_ws(p, (char*)workspace, L, false);
   p.scale = b_scale; p.scale_stride = (uint32_t)b_scale_stride;
-  p.out_scale = nullptr; p.res8 = nullptr; p.res_scale = nullptr; p.res_stride = 0;
   const uint32_t as = (uint32_t)a_scale_stride;
   switch (out_dtype) {
     case TSB200_F32: return dispatch_sddmm_fp8<float>(p, a8, out, st, a_scale, as);

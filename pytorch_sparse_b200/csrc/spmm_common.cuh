@@ -1,5 +1,6 @@
 // spmm_common.cuh — pieces shared by the SpMM forward (spmm_fw.cu) and the row-wise SDDMM (spmm_bw.cu):
-// work-queue records, kernel parameters, the per-warp cp.async index ring and the 16-byte vector math.
+// work-queue records, kernel parameters, the row-deferral rule, the per-warp cp.async index ring and the 16-byte
+// vector math.
 #pragma once
 
 #include <cstdlib>
@@ -70,6 +71,22 @@ struct SpmmParams {
   const float* res_scale;
   uint32_t res_stride;
 };
+
+// ---- the deferral rule of the row-split kernels -------------------------------------------------
+// Whether this lane's row (deg nnz) of a work item goes to the segment list instead of being walked by the item's
+// warp: it is longer than kLongT, or it lies past the item's kItemCap-nnz budget (a prefix sum over the lanes of the
+// degrees of the rows that are not long). Called by all 32 lanes. The SpMM forward's main kernels, its plan kernel
+// and the row-wise SDDMM all defer by this one rule, so planned and unplanned products walk the same rows.
+__device__ __forceinline__ bool defer_row(int deg, int lane) {
+  const bool is_long = deg > kLongT;
+  int cum = is_long ? 0 : deg;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, cum, off);
+    if (lane >= off) cum += t;
+  }
+  return (deg > 0) && (is_long || cum > kItemCap);
+}
 
 // ---- per-warp streaming index ring ------------------------------------------------------------
 template <typename T> struct IndexRing {
@@ -334,6 +351,16 @@ static inline WsLayout ws_layout(int64_t B, int64_t K, int64_t E, bool arg, bool
   L.total = off;
   return L;
 }
+// binds an unplanned workspace (layout L at ws) to p: work counters, segment queue, long rows, partials; no plan
+static inline void bind_ws(SpmmParams& p, char* ws, const WsLayout& L, bool arg) {
+  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
+  p.counters = (unsigned int*)(ws + L.counters);
+  p.segs = (Segment*)(ws + L.segs);
+  p.longs = (LongRow*)(ws + L.longs);
+  p.part_val = ws + L.part_val;
+  p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
+  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+}
 
 static inline int grid_for(const void* kernel, int threads) {
   int per_sm = 0;
@@ -358,15 +385,19 @@ struct GridCache {
   }
 };
 
-// TSB200_SPMM_ITEM_SHIFT = 0..5, read on every call, fixes the work item of the SpMM forward and SDDMM row kernels at
-// 2^s rows: a test knob, so that small matrices can run every item size. Unset or out of range: -1 (the launch's own
-// choice stands).
-static inline int item_shift_override() {
+// Work item of the SpMM forward and SDDMM row kernels: 2^s consecutive rows, s <= 5. Small matrices shrink it, so that
+// each of the grid_main * kWarpsPerCta resident warps gets at least two items of the `rows` rows (all batches).
+// TSB200_SPMM_ITEM_SHIFT = 0..5, read on every call, fixes s instead: a test knob, so that small matrices can run
+// every item size. Unset or out of range, it is ignored.
+static inline int item_shift_for(int64_t rows, int grid_main) {
+  const int64_t want = rows / ((int64_t)grid_main * kWarpsPerCta * 2);
+  int s = 0;
+  while (s < 5 && ((int64_t)2 << s) <= want) s++;
   const char* ev = getenv("TSB200_SPMM_ITEM_SHIFT");
-  if (!ev) return -1;
+  if (!ev) return s;
   char* end = nullptr;
   const long v = strtol(ev, &end, 10);
-  return (end != ev && *end == '\0' && v >= 0 && v <= 5) ? (int)v : -1;
+  return (end != ev && *end == '\0' && v >= 0 && v <= 5) ? (int)v : s;
 }
 
 }  // namespace tsb

@@ -28,6 +28,11 @@
 
 namespace tsb {
 
+// arg_out of one column from an engine's arg slot (0x7fffffff: no entry won): the winner's nnz index, or the sentinel
+// E. A row store passes E itself for an empty row (`count > 0 ? stored_arg(..) : E`); with that test in here the
+// compiler lays the stores out differently.
+__device__ __forceinline__ int64_t stored_arg(int a, int64_t E) { return a != 0x7fffffff ? (int64_t)a : E; }
+
 // T = value / output type, X = dense-operand type: T itself, or __nv_fp8_e4m3 (tsb200_spmm_fw_fp8), in which case
 // every entry's weight is fl32(value * scale[col]) and a 16-byte gather carries 16 columns.
 template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct RowEngine {
@@ -224,8 +229,8 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
 #pragma unroll
         for (int i = 0; i < VEC; i += 2) {
           longlong2 a2;
-          a2.x = (count > 0 && arg[ch * VEC + i] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i] : E;
-          a2.y = (count > 0 && arg[ch * VEC + i + 1] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i + 1] : E;
+          a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
+          a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
           stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
         }
       }
@@ -274,8 +279,8 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
 #pragma unroll
         for (int i = 0; i < VEC; i += 2) {
           longlong2 a2;
-          a2.x = (count > 0 && arg[ch * VEC + i] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i] : E;
-          a2.y = (count > 0 && arg[ch * VEC + i + 1] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i + 1] : E;
+          a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
+          a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
           stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
         }
       }
@@ -458,8 +463,8 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
 #pragma unroll
       for (int i = 0; i < VEC; i += 2) {
         longlong2 a2;
-        a2.x = (count > 0 && arg[ch * VEC + i] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i] : E;
-        a2.y = (count > 0 && arg[ch * VEC + i + 1] != 0x7fffffff) ? (int64_t)arg[ch * VEC + i + 1] : E;
+        a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
+        a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
         stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
       }
     }
@@ -478,17 +483,17 @@ template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, cons
   }
 }
 
-// column kk of a multi-segment row: its partials folded in segment order (min/max: the smallest e wins ties), the
-// mean's division applied. CG: read past L1 (partials written by other SMs during the same launch). RES: plus the
-// row's residual (scale rs) in that column.
+// column kk of a multi-segment row (nseg segments, count = its degree): its partials folded in segment order (min/max:
+// the smallest e wins ties), the mean's division applied. CG: read past L1 (partials written by other SMs during the
+// same launch). RES: plus the row's residual (scale rs) in that column. The one definition of the fold: every combine
+// of the SpMM forward calls it.
 template <int RED, bool CG, bool RES = false>
 __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow& L, int nseg, int64_t count,
                                              int64_t kk, int64_t& ar, float rs = 0.f) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const float* pv = (const float*)p.part_val;
   float a = CG ? __ldcg(pv + L.first_slot * p.K + kk) : pv[L.first_slot * p.K + kk];
-  ar = 0;
-  if (ARG) ar = CG ? __ldcg(p.part_arg + L.first_slot * p.K + kk) : p.part_arg[L.first_slot * p.K + kk];
+  int64_t r = ARG ? (CG ? __ldcg(p.part_arg + L.first_slot * p.K + kk) : p.part_arg[L.first_slot * p.K + kk]) : 0;
   for (int sgi = 1; sgi < nseg; sgi++) {
     const float v = CG ? __ldcg(pv + (L.first_slot + sgi) * p.K + kk) : pv[(L.first_slot + sgi) * p.K + kk];
     if (RED == R_SUM) a += v;
@@ -496,10 +501,11 @@ __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow&
       const int64_t va = CG ? __ldcg(p.part_arg + (L.first_slot + sgi) * p.K + kk)
                             : p.part_arg[(L.first_slot + sgi) * p.K + kk];
       const bool better = (RED == R_MIN) ? (v < a) : (v > a);
-      if (better || (v == a && va < ar)) { a = v; ar = va; }
+      if (better || (v == a && va < r)) { a = v; r = va; }
     }
   }
-  if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
+  ar = r;
+  if (RED == R_SUM && p.mean) a = a / (float)(count != 0 ? count : 1);
   if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
   return a;
 }
@@ -515,19 +521,8 @@ __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const Long
   for (int k = lane; k < kcols; k += 32) {
     const int64_t kk = p.k0 + k;
     if (kk >= p.K) break;
-    float a = __ldcg((const float*)p.part_val + L.first_slot * p.K + kk);
-    int64_t ar = ARG ? __ldcg(p.part_arg + L.first_slot * p.K + kk) : 0;
-    for (int sgi = 1; sgi < nseg; sgi++) {
-      const float v = __ldcg((const float*)p.part_val + (L.first_slot + sgi) * p.K + kk);
-      if (RED == R_SUM) a += v;
-      else {
-        const int64_t va = __ldcg(p.part_arg + (L.first_slot + sgi) * p.K + kk);
-        const bool better = (RED == R_MIN) ? (v < a) : (v > a);
-        if (better || (v == a && va < ar)) { a = v; ar = va; }
-      }
-    }
-    if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
-    if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
+    int64_t ar;
+    const float a = combine_col<RED, true, RES>(p, L, nseg, count, kk, ar, rs);
     ((T*)p.out)[L.row_b * p.K + kk] = Traits<T>::from_acc(a);
     if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
   }
@@ -559,6 +554,56 @@ __device__ __forceinline__ void combine_row_warp_q8(const SpmmParams& p, const L
     const float a = combine_col<RED, true, RES>(p, L, nseg, count, kk, ar, rs);
     ((uint8_t*)p.out)[L.row_b * p.K + kk] = e4m3_quant(a, s);
     if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
+  }
+}
+
+// queue a row deferred by defer_row (row r0 + lane of batch b, nnz [rp0, rp1), deg = rp1 - rp0) as segments of
+// <= kSeg nnz; a row of several segments also gets a LongRow and one partial slot per segment, for the combine
+__device__ __forceinline__ void push_row_segments(const SpmmParams& p, int64_t b, int64_t r0, int lane, int64_t rp0,
+                                                  int64_t rp1, int deg) {
+  const int nseg = (deg + kSeg - 1) / kSeg;
+  const unsigned seg0 = atomicAdd(&p.counters[1], (unsigned)nseg);
+  int64_t slot0 = -1;
+  if (nseg > 1) {
+    slot0 = atomicAdd(&p.counters[3], (unsigned)nseg);
+    const unsigned lr = atomicAdd(&p.counters[2], 1u);
+    if ((int64_t)lr < p.long_cap) {
+      LongRow L;
+      L.row_b = b * p.M + r0 + lane;
+      L.first_slot = slot0;
+      L.nseg_count = ((int64_t)nseg << 40) | (int64_t)deg;
+      p.longs[lr] = L;
+    }
+  }
+  for (int sgi = 0; sgi < nseg; sgi++) {
+    if ((int64_t)seg0 + sgi < p.seg_cap) {
+      Segment S;
+      S.row_b = b * p.M + r0 + lane;
+      S.start = rp0 + (int64_t)sgi * kSeg;
+      S.end = min(rp1, S.start + kSeg);
+      S.slot = slot0 < 0 ? -1 : slot0 + sgi;
+      p.segs[seg0 + sgi] = S;
+    }
+  }
+}
+
+// the fp32 partial of one segment of a multi-segment row, and its arg slots (min / max), into partial slot `slot`;
+// written by group 0 after reduce_groups
+template <int LPR, typename Eng, int CH>
+__device__ __forceinline__ void store_partial(const SpmmParams& p, const Eng& eng, int64_t slot,
+                                              const bool (&col_ok)[CH], int li) {
+  constexpr int VEC = Eng::VEC;
+  float* pv = (float*)p.part_val + slot * p.K + p.k0;
+  int64_t* pa = Eng::ARG ? p.part_arg + slot * p.K + p.k0 : nullptr;
+#pragma unroll
+  for (int ch = 0; ch < CH; ch++) {
+    if (!col_ok[ch]) continue;
+    const int koff = (ch * LPR + li) * VEC;
+#pragma unroll
+    for (int i = 0; i < VEC; i++) {
+      pv[koff + i] = eng.acc_float(ch * VEC + i);
+      if (Eng::ARG) pa[koff + i] = stored_arg(eng.arg[ch * VEC + i], p.E);
+    }
   }
 }
 
@@ -622,43 +667,9 @@ spmm_vec_kernel(const SpmmParams p) {
       const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
       defer_mask = (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
     } else {
-      // nnz budget: prefix sum of the degrees of the non-long rows
-      const bool is_long = deg > kLongT;
-      int cum = is_long ? 0 : deg;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, cum, off);
-        if (lane >= off) cum += t;
-      }
-      const bool defer = (deg > 0) && (is_long || cum > kItemCap);
+      const bool defer = defer_row(deg, lane);
       defer_mask = __ballot_sync(0xffffffffu, defer);
-
-      if (defer) {  // rare: push this row's segments
-        const int nseg = (deg + kSeg - 1) / kSeg;
-        const unsigned seg0 = atomicAdd(&p.counters[1], (unsigned)nseg);
-        int64_t slot0 = -1;
-        if (nseg > 1) {
-          slot0 = atomicAdd(&p.counters[3], (unsigned)nseg);
-          const unsigned lr = atomicAdd(&p.counters[2], 1u);
-          if ((int64_t)lr < p.long_cap) {
-            LongRow L;
-            L.row_b = b * p.M + r0 + lane;
-            L.first_slot = slot0;
-            L.nseg_count = ((int64_t)nseg << 40) | (int64_t)deg;
-            p.longs[lr] = L;
-          }
-        }
-        for (int sgi = 0; sgi < nseg; sgi++) {
-          if ((int64_t)seg0 + sgi < p.seg_cap) {
-            Segment S;
-            S.row_b = b * p.M + r0 + lane;
-            S.start = rp0 + (int64_t)sgi * kSeg;
-            S.end = min(rp1, S.start + kSeg);
-            S.slot = slot0 < 0 ? -1 : slot0 + sgi;
-            p.segs[seg0 + sgi] = S;
-          }
-        }
-      }
+      if (defer) push_row_segments(p, b, r0, lane, rp0, rp1, deg);  // rare
     }
     __syncwarp();
 
@@ -729,20 +740,7 @@ spmm_vec_kernel(const SpmmParams p) {
                                         RES ? res_scale(p, row) : 0.f);
         }
       } else {
-        if (g == 0) {
-          float* pv = (float*)p.part_val + S.slot * p.K + p.k0;
-          int64_t* pa = Eng::ARG ? p.part_arg + S.slot * p.K + p.k0 : nullptr;
-#pragma unroll
-          for (int ch = 0; ch < CH; ch++) {
-            if (!col_ok[ch]) continue;
-            const int koff = (ch * LPR + li) * VEC;
-#pragma unroll
-            for (int i = 0; i < VEC; i++) {
-              pv[koff + i] = eng.acc_float(ch * VEC + i);
-              if (Eng::ARG) pa[koff + i] = eng.arg[ch * VEC + i] == 0x7fffffff ? p.E : (int64_t)eng.arg[ch * VEC + i];
-            }
-          }
-        }
+        if (g == 0) store_partial<LPR>(p, eng, S.slot, col_ok, li);
         __syncwarp();
         __threadfence();  // this segment's partial is visible before its completion is counted
         const uint32_t lr = __ldg(p.seg_lr + sidx);
@@ -821,42 +819,9 @@ spmm_gpr_kernel(const SpmmParams p) {
       const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
       defer_mask = (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
     } else {
-      const bool is_long = deg > kLongT;
-      int cum = is_long ? 0 : deg;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, cum, off);
-        if (lane >= off) cum += t;
-      }
-      const bool defer = (deg > 0) && (is_long || cum > kItemCap);
+      const bool defer = defer_row(deg, lane);
       defer_mask = __ballot_sync(0xffffffffu, defer);
-      if (defer) {
-        const int nseg = (deg + kSeg - 1) / kSeg;
-        const unsigned seg0 = atomicAdd(&p.counters[1], (unsigned)nseg);
-        int64_t slot0 = -1;
-        if (nseg > 1) {
-          slot0 = atomicAdd(&p.counters[3], (unsigned)nseg);
-          const unsigned lr = atomicAdd(&p.counters[2], 1u);
-          if ((int64_t)lr < p.long_cap) {
-            LongRow L;
-            L.row_b = b * p.M + r0 + lane;
-            L.first_slot = slot0;
-            L.nseg_count = ((int64_t)nseg << 40) | (int64_t)deg;
-            p.longs[lr] = L;
-          }
-        }
-        for (int sgi = 0; sgi < nseg; sgi++) {
-          if ((int64_t)seg0 + sgi < p.seg_cap) {
-            Segment S;
-            S.row_b = b * p.M + r0 + lane;
-            S.start = rp0 + (int64_t)sgi * kSeg;
-            S.end = min(rp1, S.start + kSeg);
-            S.slot = slot0 < 0 ? -1 : slot0 + sgi;
-            p.segs[seg0 + sgi] = S;
-          }
-        }
-      }
-    
+      if (defer) push_row_segments(p, b, r0, lane, rp0, rp1, deg);
     }
     __syncwarp();
 
@@ -1001,18 +966,7 @@ spmm_seg_kernel(const SpmmParams p) {
                         ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0,
                         RES ? res_row(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
       } else {
-        float* pv = (float*)p.part_val + S.slot * p.K + p.k0;
-        int64_t* pa = Eng::ARG ? p.part_arg + S.slot * p.K + p.k0 : nullptr;
-#pragma unroll
-        for (int ch = 0; ch < CH; ch++) {
-          if (!col_ok[ch]) continue;
-          const int koff = (ch * LPR + li) * VEC;
-#pragma unroll
-          for (int i = 0; i < VEC; i++) {
-            pv[koff + i] = eng.acc_float(ch * VEC + i);
-            if (Eng::ARG) pa[koff + i] = eng.arg[ch * VEC + i] == 0x7fffffff ? p.E : (int64_t)eng.arg[ch * VEC + i];
-          }
-        }
+        store_partial<LPR>(p, eng, S.slot, col_ok, li);
       }
     }
     __syncwarp();
@@ -1032,19 +986,8 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
     for (int k = threadIdx.x; k < kcols; k += blockDim.x) {
       const int64_t kk = p.k0 + k;
       if (kk >= p.K) break;
-      float a = ((const float*)p.part_val)[L.first_slot * p.K + kk];
-      int64_t ar = ARG ? p.part_arg[L.first_slot * p.K + kk] : 0;
-      for (int sgi = 1; sgi < nseg; sgi++) {
-        const float v = ((const float*)p.part_val)[(L.first_slot + sgi) * p.K + kk];
-        if (RED == R_SUM) a += v;
-        else {
-          const int64_t va = p.part_arg[(L.first_slot + sgi) * p.K + kk];
-          const bool better = (RED == R_MIN) ? (v < a) : (v > a);
-          if (better || (v == a && va < ar)) { a = v; ar = va; }
-        }
-      }
-      if (RED == R_SUM && p.mean) a = a / (float)(count > 0 ? count : 1);
-      if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
+      int64_t ar;
+      float a = combine_col<RED, false, RES>(p, L, nseg, count, kk, ar, rs);
       if (RED == R_SUM && p.acc_mode) {
         float* pr = p.partial + L.row_b * p.K + kk;
         if (p.acc_mode != 1) a += *pr;
@@ -1182,12 +1125,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
   auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO, RES>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
-  // small matrices: shrink the work item so that every resident warp gets rows
-  int64_t want = p.M * p.B / ((int64_t)grid_main * kWarpsPerCta * 2);
-  p.item_shift = 0;
-  while (p.item_shift < 5 && ((int64_t)2 << p.item_shift) <= want) p.item_shift++;
-  const int forced_shift = item_shift_override();  // tests: every item size on a small matrix
-  if (forced_shift >= 0) p.item_shift = forced_shift;
+  p.item_shift = item_shift_for(p.M * p.B, grid_main);
   const int64_t n_items = ((p.M + (1 << p.item_shift) - 1) >> p.item_shift) * p.B;
   for (int k0 = 0; k0 < p.K; k0 += kcols) {
     p.k0 = k0;
@@ -1277,8 +1215,8 @@ static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
 }
 
 // ---- plan: the segment list of a matrix, built once (tsb200_spmm_plan) -----------------------------------------
-// One warp per group of 32 rows, the same rule as the unplanned main kernels (rows longer than kLongT nnz, and rows
-// beyond the group's kItemCap-nnz budget, become <= kSeg-nnz segments); also leaves one mask word per group.
+// One warp per group of 32 rows: the rows defer_row defers become <= kSeg-nnz segments; also leaves one mask word per
+// group. Its push writes the records of push_row_segments from 64-bit degrees, plus each segment's long row (seg_lr).
 __global__ void __launch_bounds__(256)
 spmm_plan_kernel(const int64_t* __restrict__ rowptr, int64_t M, uint32_t* __restrict__ mask, Segment* __restrict__ segs,
                  uint32_t* __restrict__ seg_lr, LongRow* __restrict__ longs, unsigned int* __restrict__ counters,
@@ -1293,15 +1231,7 @@ spmm_plan_kernel(const int64_t* __restrict__ rowptr, int64_t M, uint32_t* __rest
     const int64_t rp0 = __ldg(rowptr + r0 + min(lane, nrows));
     const int64_t rp1 = __ldg(rowptr + r0 + min(lane + 1, nrows));
     const int64_t deg64 = rp1 - rp0;
-    const int deg = (int)min(deg64, (int64_t)0x3fffffff);
-    const bool is_long = deg > kLongT;
-    int cum = is_long ? 0 : deg;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, cum, off);
-      if (lane >= off) cum += t;
-    }
-    const bool defer = (deg > 0) && (is_long || cum > kItemCap);
+    const bool defer = defer_row((int)min(deg64, (int64_t)0x3fffffff), lane);
     const unsigned defer_mask = __ballot_sync(0xffffffffu, defer);
     if (lane == 0) mask[grp] = defer_mask;
     if (defer) {
@@ -1366,6 +1296,30 @@ static inline PlannedWs planned_ws(int64_t K, int64_t n_long, int64_t n_slot, bo
   L.total = off;
   return L;
 }
+// checks a plan of p.M rows and p.E nnz (tsb200_spmm_plan, with its counts) and its planned workspace, then binds
+// both to p: 0 or the error code
+static int bind_plan(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                     int64_t n_slot, void* workspace, size_t workspace_bytes, bool arg) {
+  const PlanLayout PL = plan_layout(p.M, p.E);
+  if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
+  if (n_seg > PL.seg_cap || n_long > PL.long_cap || ((uintptr_t)plan & 255)) return TSB200_ERR_INVALID_ARG;
+  const PlannedWs W = planned_ws(p.K, n_long, n_slot, arg);
+  if (!workspace || workspace_bytes < W.total) return TSB200_ERR_WORKSPACE;
+  if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
+  char* ws = (char*)workspace;
+  const char* pl = (const char*)plan;
+  p.counters = (unsigned int*)(ws + W.counters);
+  p.long_done = (uint32_t*)(ws + W.long_done);   // directly behind the counters: one memset clears both
+  p.segs = (Segment*)(pl + PL.segs);
+  p.longs = (LongRow*)(pl + PL.longs);
+  p.seg_lr = (const uint32_t*)(pl + PL.seg_lr);
+  p.plan_mask = (const uint32_t*)(pl + PL.mask);
+  p.n_seg = n_seg; p.n_long = n_long;
+  p.part_val = ws + W.part_val;
+  p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
+  p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
+  return 0;
+}
 
 template <typename T, int RED>
 static int launch_generic(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
@@ -1410,18 +1364,8 @@ extern "C" int tsb200_spmm_fw(const int64_t* rowptr, const int64_t* col, const v
     const WsLayout L = ws_layout(B, K, E, arg);
     if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
     if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
-    char* ws = (char*)workspace;
-    SpmmParams p;
-    p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
-    p.B = B; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
-    p.partial = nullptr; p.acc_mode = 0;
-    p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-    p.counters = (unsigned int*)(ws + L.counters);
-    p.segs = (Segment*)(ws + L.segs);
-    p.longs = (LongRow*)(ws + L.longs);
-    p.part_val = ws + L.part_val;
-    p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
-    p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+    SpmmParams p{rowptr, col, value, mat, out, arg_out, B, M, N, K, E};
+    bind_ws(p, (char*)workspace, L, arg);
     switch (dtype) {
       case TSB200_F32: return dispatch_red_vec<float>(p, reduce, st);
       case TSB200_F16: return dispatch_red_vec<__half>(p, reduce, st);
@@ -1459,18 +1403,9 @@ extern "C" int tsb200_spmm_fw_acc(const int64_t* rowptr, const int64_t* col, con
   const WsLayout L = ws_layout(B, K, E, false);
   if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
   if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
-  char* ws = (char*)workspace;
-  SpmmParams p;
-  p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = nullptr;
-  p.B = B; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
+  SpmmParams p{rowptr, col, value, mat, out, nullptr, B, M, N, K, E};
   p.partial = partial; p.acc_mode = acc_mode;
-  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-  p.counters = (unsigned int*)(ws + L.counters);
-  p.segs = (Segment*)(ws + L.segs);
-  p.longs = (LongRow*)(ws + L.longs);
-  p.part_val = ws + L.part_val;
-  p.part_arg = nullptr;
-  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+  bind_ws(p, (char*)workspace, L, false);
   switch (dtype) {
     case TSB200_F32: return dispatch_shape<float, R_SUM, true>(p, st);
     case TSB200_F16: return dispatch_shape<__half, R_SUM, true>(p, st);
@@ -1530,29 +1465,9 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
   if (M * K == 0) return 0;
   if (!rowptr || !col || !mat || !out || !plan || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
   if (!vec_eligible(dtype, K, E, N, value, mat, out, col, arg_out)) return TSB200_ERR_UNSUPPORTED;
-  const PlanLayout PL = plan_layout(M, E);
-  if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
-  if (n_seg > PL.seg_cap || n_long > PL.long_cap) return TSB200_ERR_INVALID_ARG;
-  const PlannedWs W = planned_ws(K, n_long, n_slot, arg);
-  if (!workspace || workspace_bytes < W.total) return TSB200_ERR_WORKSPACE;
-  if (((uintptr_t)workspace & 255) || ((uintptr_t)plan & 255)) return TSB200_ERR_INVALID_ARG;
+  SpmmParams p{rowptr, col, value, mat, out, arg_out, 1, M, N, K, E};
+  if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  const char* pl = (const char*)plan;
-  SpmmParams p;
-  p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
-  p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
-  p.partial = nullptr; p.acc_mode = 0;
-  p.counters = (unsigned int*)(ws + W.counters);
-  p.long_done = (uint32_t*)(ws + W.long_done);   // directly behind the counters: one memset clears both
-  p.segs = (Segment*)(pl + PL.segs);
-  p.longs = (LongRow*)(pl + PL.longs);
-  p.seg_lr = (const uint32_t*)(pl + PL.seg_lr);
-  p.plan_mask = (const uint32_t*)(pl + PL.mask);
-  p.n_seg = n_seg; p.n_long = n_long;
-  p.part_val = ws + W.part_val;
-  p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
-  p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
   switch (dtype) {
     case TSB200_F32: return dispatch_red_vec<float, true>(p, reduce, st);
     case TSB200_F16: return dispatch_red_vec<__half, true>(p, reduce, st);
@@ -1637,7 +1552,9 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
   if (!rowptr || !out || (QO && !out_scale) || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
   if (QO && ((uintptr_t)out_scale & 3)) return TSB200_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
-  SpmmParams p;
+  SpmmParams p{rowptr, col, value, mat, out, arg_out, 1, M, N, K, E};
+  p.scale = scale; p.scale_stride = (uint32_t)scale_stride;
+  p.out_scale = out_scale;
   p.res8 = res8; p.res_scale = res_scale; p.res_stride = (uint32_t)res_stride;
   if (res8) {
     if (!res_scale || (res_stride != 0 && res_stride != 1)) return TSB200_ERR_INVALID_ARG;
@@ -1645,7 +1562,6 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
     if (((uintptr_t)res8 & 15) || ((uintptr_t)res_scale & 3)) return TSB200_ERR_UNSUPPORTED;
     if (E == 0 && K > 0) {  // every row is empty: the result is the residual alone
       if ((uintptr_t)out & 15) return TSB200_ERR_UNSUPPORTED;
-      p.out = out; p.out_scale = out_scale; p.M = M; p.K = K; p.k0 = 0;
       if constexpr (QO) return launch_res_only<float, true>(p, st);
       switch (out_dtype) {
         case TSB200_F32: return launch_res_only<float, false>(p, st);
@@ -1672,41 +1588,14 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
     return TSB200_ERR_UNSUPPORTED;
   if ((value && ((uintptr_t)value & 3)) || (arg_out && ((uintptr_t)arg_out & 15))) return TSB200_ERR_UNSUPPORTED;
   if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
-  char* ws = (char*)workspace;
-  p.rowptr = rowptr; p.col = col; p.value = value; p.mat = mat; p.out = out; p.arg_out = arg_out;
-  p.B = 1; p.M = M; p.N = N; p.K = K; p.E = E; p.k0 = 0; p.mean = 0; p.item_shift = 5;
-  p.partial = nullptr; p.acc_mode = 0;
-  p.scale = scale; p.scale_stride = (uint32_t)scale_stride;
-  p.out_scale = out_scale;
   if (plan) {  // planned: the layout of tsb200_spmm_fw_planned
-    const PlanLayout PL = plan_layout(M, E);
-    if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
-    if (n_seg > PL.seg_cap || n_long > PL.long_cap || ((uintptr_t)plan & 255)) return TSB200_ERR_INVALID_ARG;
-    const PlannedWs W = planned_ws(K, n_long, n_slot, arg);
-    if (workspace_bytes < W.total) return TSB200_ERR_WORKSPACE;
-    const char* pl = (const char*)plan;
-    p.counters = (unsigned int*)(ws + W.counters);
-    p.long_done = (uint32_t*)(ws + W.long_done);
-    p.segs = (Segment*)(pl + PL.segs);
-    p.longs = (LongRow*)(pl + PL.longs);
-    p.seg_lr = (const uint32_t*)(pl + PL.seg_lr);
-    p.plan_mask = (const uint32_t*)(pl + PL.mask);
-    p.n_seg = n_seg; p.n_long = n_long;
-    p.part_val = ws + W.part_val;
-    p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
-    p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
+    if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)) return rc;
     return dispatch_fp8_res<true, QO>(p, out_dtype, reduce, st);
   }
   // unplanned: the layout of tsb200_spmm_fw (tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce))
   const WsLayout L = ws_layout(1, K, E, arg);
   if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-  p.plan_mask = nullptr; p.seg_lr = nullptr; p.long_done = nullptr; p.n_seg = 0; p.n_long = 0;
-  p.counters = (unsigned int*)(ws + L.counters);
-  p.segs = (Segment*)(ws + L.segs);
-  p.longs = (LongRow*)(ws + L.longs);
-  p.part_val = ws + L.part_val;
-  p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
-  p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
+  bind_ws(p, (char*)workspace, L, arg);
   return dispatch_fp8_res<false, QO>(p, out_dtype, reduce, st);
 }
 }  // namespace tsb

@@ -191,22 +191,33 @@ def spmm_fw(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor,
         return out, arg_out
     with _on_device(dev):
         plannable = B == 1 and dt in (0, 2, 3) and (K * mat.element_size()) % 16 == 0
-        if plan is None and plannable:
-            plan = _auto_plan(rowptr, E)
-        if plan is not None and plannable and plan.M == M and plan.E == E:
-            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
-            ws = _workspace(nws, dev)
+        pl, ws, nws = _plan_workspace(plan, plannable, rowptr, B, M, K, E, dt, red, dev)
+        if pl[0] is not None:
             rc = lib.tsb200_spmm_fw_planned(_p(rowptr), _p(col), _p(value), _p(mat), _p(out), _p(arg_out), M, N, K, E,
-                                            dt, red, _p(plan.data), plan.data.numel(), plan.n_seg, plan.n_long,
-                                            plan.n_slot, _p(ws), nws, _stream(dev))
+                                            dt, red, *pl, _p(ws), nws, _stream(dev))
             if rc != -2:   # TSB200_ERR_UNSUPPORTED (alignment): fall through to the unplanned call
                 check(rc, "tsb200_spmm_fw_planned")
                 return out, arg_out
-        nws = lib.tsb200_spmm_fw_workspace_bytes(B, M, K, E, dt, red)
-        ws = _workspace(nws, dev)
+            pl, ws, nws = _plan_workspace(None, False, rowptr, B, M, K, E, dt, red, dev)
         check(lib.tsb200_spmm_fw(_p(rowptr), _p(col), _p(value), _p(mat), _p(out), _p(arg_out),
                                  B, M, N, K, E, dt, red, _p(ws), nws, _stream(dev)), "tsb200_spmm_fw")
     return out, arg_out
+
+
+def _plan_workspace(plan: Optional[SpmmPlan], plannable: bool, rowptr: Tensor, B: int, M: int, K: int, E: int,
+                    dt: int, red: int, dev: torch.device):
+    """The plan and the workspace of one SpMM forward. A plannable product uses the given plan, else the one cached
+    for `rowptr`, and only if it was built for these M and E. Returns (plan arguments, workspace, workspace bytes);
+    the plan arguments are (plan, plan_bytes, n_seg, n_long, n_slot), with plan None for an unplanned call."""
+    if plannable and plan is None:
+        plan = _auto_plan(rowptr, E)
+    if plannable and plan is not None and plan.M == M and plan.E == E:
+        nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
+        pl = (_p(plan.data), plan.data.numel(), plan.n_seg, plan.n_long, plan.n_slot)
+    else:
+        nws = lib.tsb200_spmm_fw_workspace_bytes(B, M, K, E, dt, red)
+        pl = (None, 0, 0, 0, 0)
+    return pl, _workspace(nws, dev), nws
 
 
 _FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
@@ -294,33 +305,20 @@ def _fp8_residual(what: str, residual: Optional[Tensor], residual_scale: Optiona
     return residual, residual_scale.contiguous(), stride
 
 
-def _fp8_res_call(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor, stride: int, res,
-                  out: Tensor, out_scale: Optional[Tensor], dt: int, red: int, plan: Optional[SpmmPlan]) -> None:
-    """tsb200_spmm_fw_fp8_res: out_dtype code `dt` result, or an e4m3 result when out_scale is given (dt = float32)."""
-    residual, residual_scale, rstride = res
+def _fp8_call(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor, stride: int, res,
+              out: Tensor, out_scale: Optional[Tensor], arg_out: Optional[Tensor], dt: int, red: int,
+              plan: Optional[SpmmPlan]) -> None:
+    """tsb200_spmm_fw_fp8_res: out_dtype code `dt` result, or an e4m3 result when out_scale is given (dt = float32).
+    Without a residual (res None) it is tsb200_spmm_fw_fp8 / tsb200_spmm_fw_fp8_quant."""
+    residual, residual_scale, rstride = res if res is not None else (None, None, 0)
     N, K = x8.shape
     M, E = rowptr.numel() - 1, col.numel()
     dev = x8.device
     with _on_device(dev):
-        plan = _fp8_plan(plan, rowptr, M, E) if E > 0 else None
-        if plan is not None:
-            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
-            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
-        else:
-            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, dt, red)
-            pl, pl_bytes, counts = None, 0, (0, 0, 0)
-        ws = _workspace(nws, dev)
+        pl, ws, nws = _plan_workspace(plan, E > 0, rowptr, 1, M, K, E, dt, red, dev)
         check(lib.tsb200_spmm_fw_fp8_res(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(residual),
-                                         _p(residual_scale), rstride, _p(out), _p(out_scale), None, M, N, K, E, dt, red,
-                                         pl, pl_bytes, *counts, _p(ws), nws, _stream(dev)), "tsb200_spmm_fw_fp8_res")
-
-
-def _fp8_plan(plan: Optional[SpmmPlan], rowptr: Tensor, M: int, E: int) -> Optional[SpmmPlan]:
-    if plan is None:
-        plan = _auto_plan(rowptr, E)
-    if plan is not None and (plan.M != M or plan.E != E):
-        plan = None
-    return plan
+                                         _p(residual_scale), rstride, _p(out), _p(out_scale), _p(arg_out), M, N, K, E,
+                                         dt, red, *pl, _p(ws), nws, _stream(dev)), "tsb200_spmm_fw_fp8_res")
 
 
 def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor, scale: Tensor,
@@ -337,7 +335,7 @@ def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor
     result is round_out(fl32(y + fl32(residual_scale[m] * residual[m]))) with y the float32 result."""
     rowptr, col, value, scale, stride = _fp8_args("spmm_fp8", rowptr, col, value, x8, scale, out_dtype)
     red = _reduce_code(reduce)
-    N, K = x8.shape
+    K = x8.size(1)
     M, E = rowptr.numel() - 1, col.numel()
     res = _fp8_residual("spmm_fp8", residual, residual_scale, x8, M, red)
     dev = x8.device
@@ -345,26 +343,12 @@ def spmm_fw_fp8(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: Tensor
     arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
     if out.numel() == 0:
         return out, arg_out
-    if res is not None:
-        _fp8_res_call(rowptr, col, value, x8, scale, stride, res, out, None, _FP8_OUT[out_dtype], red, plan)
-        return out, arg_out
-    if E == 0:
+    if res is None and E == 0:
         out.zero_()
         if arg_out is not None:
             arg_out.fill_(0)
         return out, arg_out
-    with _on_device(dev):
-        plan = _fp8_plan(plan, rowptr, M, E)
-        if plan is not None:
-            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
-            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
-        else:
-            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, _FP8_OUT[out_dtype], red)
-            pl, pl_bytes, counts = None, 0, (0, 0, 0)
-        ws = _workspace(nws, dev)
-        check(lib.tsb200_spmm_fw_fp8(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(out), _p(arg_out),
-                                     M, N, K, E, _FP8_OUT[out_dtype], red, pl, pl_bytes, *counts, _p(ws), nws,
-                                     _stream(dev)), "tsb200_spmm_fw_fp8")
+    _fp8_call(rowptr, col, value, x8, scale, stride, res, out, None, arg_out, _FP8_OUT[out_dtype], red, plan)
     return out, arg_out
 
 
@@ -382,7 +366,7 @@ def spmm_fw_fp8_quant(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: 
     `residual` (e4m3 [M, K]) with `residual_scale` (float32 [] or [M]), sum / mean only (tsb200_spmm_fw_fp8_res):
     the rows quantised are z = fl32(y + fl32(residual_scale[m] * residual[m])) instead of y."""
     rowptr, col, value, scale, stride = _fp8_args("spmm_fp8_quant", rowptr, col, value, x8, scale, None)
-    N, K = x8.shape
+    K = x8.size(1)
     if K > FP8_QUANT_MAX_K:
         raise RuntimeError(f"spmm_fp8_quant: the number of columns K = {K} must be at most {FP8_QUANT_MAX_K}")
     red = _reduce_code(reduce)
@@ -394,27 +378,13 @@ def spmm_fw_fp8_quant(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x8: 
     arg_out = torch.empty(M, K, dtype=torch.int64, device=dev) if red >= 2 else None
     if M == 0:
         return y8, y_scale, arg_out
-    if res is not None and K > 0:
-        _fp8_res_call(rowptr, col, value, x8, scale, stride, res, y8, y_scale, _FP8_OUT[torch.float32], red, plan)
-        return y8, y_scale, arg_out
-    if E == 0 or K == 0:
+    if K == 0 or (res is None and E == 0):
         y8.zero_()
         y_scale.fill_(1.0)
         if arg_out is not None:
             arg_out.fill_(0)
         return y8, y_scale, arg_out
-    with _on_device(dev):
-        plan = _fp8_plan(plan, rowptr, M, E)
-        if plan is not None:
-            nws = lib.tsb200_spmm_fw_planned_workspace_bytes(K, plan.n_long, plan.n_slot, red)
-            pl, pl_bytes, counts = _p(plan.data), plan.data.numel(), (plan.n_seg, plan.n_long, plan.n_slot)
-        else:
-            nws = lib.tsb200_spmm_fw_workspace_bytes(1, M, K, E, _FP8_OUT[torch.float32], red)
-            pl, pl_bytes, counts = None, 0, (0, 0, 0)
-        ws = _workspace(nws, dev)
-        check(lib.tsb200_spmm_fw_fp8_quant(_p(rowptr), _p(col), _p(value), _p(x8), _p(scale), stride, _p(y8),
-                                           _p(y_scale), _p(arg_out), M, N, K, E, red, pl, pl_bytes, *counts, _p(ws),
-                                           nws, _stream(dev)), "tsb200_spmm_fw_fp8_quant")
+    _fp8_call(rowptr, col, value, x8, scale, stride, res, y8, y_scale, arg_out, _FP8_OUT[torch.float32], red, plan)
     return y8, y_scale, arg_out
 
 

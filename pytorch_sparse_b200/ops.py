@@ -966,12 +966,15 @@ class SPMMMean(torch.autograd.Function):
         if ctx.has_value and ctx.needs_input_grad[3]:
             grad_value = spmm_value_bw(row, rowptr, col, mat, grad_out, "mean")
         if ctx.needs_input_grad[7]:
-            # per-nnz weight value/count(row) (or 1/count) in CSC order (csrc/spmm.cpp:166-177)
+            # per-nnz weight value/count(row) (or 1/count) in CSC order (csrc/spmm.cpp:166-177), divided in the
+            # accumulator type and rounded once to mat's dtype: the forward and grad_value divide by the exact count,
+            # which bf16 (above 256) and f16 (above 2048) cannot always hold (DESIGN §3.2)
             if row_csc is None:
                 row_csc = row.index_select(0, csr2csc)
-            cnt = rowcount.index_select(0, row_csc).to(mat.dtype).clamp_(min=1)
-            w = value.index_select(0, csr2csc).div(cnt) if ctx.has_value else cnt.reciprocal_()
-            grad_mat, _ = spmm_fw(colptr, row_csc, w, grad_out, "sum")
+            acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
+            cnt = rowcount.index_select(0, row_csc).to(acc).clamp_(min=1)
+            w = value.index_select(0, csr2csc).to(acc).div_(cnt) if ctx.has_value else cnt.reciprocal_()
+            grad_mat, _ = spmm_fw(colptr, row_csc, w.to(mat.dtype), grad_out, "sum")
         return None, None, None, grad_value, None, None, None, grad_mat, None
 
 

@@ -261,6 +261,37 @@ TSB200_API int tsb200_sddmm_fp8(const int64_t* rowptr, const int64_t* col, const
                                 size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Multi-head SpMM and SDDMM: one weight per entry and head (graph attention; no counterpart in the reference).  B = 1.
+ *   x, a, b are [rows, H, D] contiguous (row-major, K = H * D columns per row), dtype F32 / F64 / F16 / BF16.
+ *   tsb200_spmm_heads:  out[m, h, :] = sum_{e in row m} value[e, h] * x[col_e, h, :]
+ *     value dtype[E, H] or NULL (every weight 1: the plain sum over K = H * D columns); out dtype[M, H, D].
+ *     fp32 accumulation (fp64 for F64), one rounding to dtype; an empty row gives +0. With
+ *     D * sizeof(dtype) % 16 == 0 and 16-byte aligned x / out (col 8 B, value 4 B) the sum kernels of tsb200_spmm_fw
+ *     run with each 16-byte chunk weighed by its own head's value; with H == 1 the bits are those of tsb200_spmm_fw
+ *     (or tsb200_spmm_fw_planned). Otherwise a lane-per-column kernel sums every column in entry order.
+ *     plan: NULL, or tsb200_spmm_plan's plan of (rowptr, E) with its counts, as for tsb200_spmm_fw_planned.
+ *     workspace: tsb200_spmm_fw_workspace_bytes(1, M, H * D, E, dtype, TSB200_SUM) bytes without a plan,
+ *     tsb200_spmm_fw_planned_workspace_bytes(H * D, n_long, n_slot, TSB200_SUM) with one; 256 B aligned.
+ *   tsb200_sddmm_heads: out[e, h] = <a[row_e, h, :], b[col_e, h, :]>, a dtype[M, H, D], b dtype[N, H, D],
+ *     out dtype[E, H] in CSR order; fp32 accumulation (fp64 for F64), one rounding. With HL = D * sizeof(dtype) / 16
+ *     a power of two, H * HL <= 64 vectors, HL not above the row's lane count, 16-byte aligned a / b and a workspace of
+ *     tsb200_spmm_value_bw_workspace_bytes(1, M, H * D, E, dtype) bytes (256 B aligned) the row-wise kernels of
+ *     tsb200_spmm_value_bw run, each step's dot reduced over the HL lanes of its head; with H == 1 their bits are
+ *     tsb200_spmm_value_bw's (reduce SUM) wherever both take the row-wise kernel. Otherwise a warp-per-row kernel.
+ *   Nothing is launched when there is nothing to write (M * H * D == 0, resp. E * H == 0); E == 0 (spmm) or D == 0
+ *   (sddmm) writes +0. TSB200_ERR_INVALID_ARG for a negative extent or count, a NULL pointer that is needed or a
+ *   misaligned workspace; TSB200_ERR_UNSUPPORTED for another dtype or H * D >= 2^40; TSB200_ERR_WORKSPACE for a
+ *   short workspace. The workspace and plan rules are tsb200_spmm_fw_planned's.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_spmm_heads(const int64_t* rowptr, const int64_t* col, const void* value, const void* x, void* out,
+                                 int64_t M, int64_t N, int64_t H, int64_t D, int64_t E, int dtype, const void* plan,
+                                 size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+TSB200_API int tsb200_sddmm_heads(const int64_t* rowptr, const int64_t* col, const void* a, const void* b, void* out,
+                                  int64_t M, int64_t N, int64_t H, int64_t D, int64_t E, int dtype, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Fused min/max backward.  Replaces the ATen chain in SPMMMin/SPMMMax::backward
  *   (csrc/spmm.cpp:204-242, 264-302): for every (b,m,k) with a = arg_out[b,m,k] != E,
  *     grad_value[a]           += mat[b,col[a],k] * grad_out[b,m,k]      (if grad_value != NULL)

@@ -51,6 +51,11 @@ SIGNATURES = {
     "tsb200_sddmm_fp8_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
     "tsb200_sddmm_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p,
                                  c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_heads": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                  c_int64, c_int, c_void_p, c_size_t, c_int64, c_int64, c_int64, c_void_p, c_size_t,
+                                  c_void_p]),
+    "tsb200_sddmm_heads": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                   c_int64, c_int, c_void_p, c_size_t, c_void_p]),
     "tsb200_spmm_minmax_bw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "tsb200_ind2ptr": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p]),

@@ -177,7 +177,9 @@ value_bw_vec_kernel(const int64_t* __restrict__ row, const int64_t* __restrict__
 // T = output type, X = type of both dense operands: T itself, or __nv_fp8_e4m3 (tsb200_sddmm_fp8). For e4m3 a vector
 // is 16 columns, `scale` is the row operand's scale of the row, and the gathered row's scale bscale[c * bstride] is
 // loaded next to its column word; after the reduction out = round_T(fl32(fl32(scale * bscale[c]) * dot)).
-template <typename T, int LPR, int CH, int U, typename X = T> struct SddmmEngine {
+// HL > 0 (tsb200_sddmm_heads): the operands are [rows, H, D] with HL = D * sizeof(T) / 16 lanes per head (a power of
+// two, <= LPR): each step's dot is reduced over the HL lanes of a head, and out is [E, H].
+template <typename T, int LPR, int CH, int U, typename X = T, int HL = 0> struct SddmmEngine {
   static constexpr bool Q8 = !std::is_same<X, T>::value;
   static constexpr int VEC = 16 / sizeof(X);
   static constexpr int G = 32 / LPR;
@@ -221,41 +223,80 @@ template <typename T, int LPR, int CH, int U, typename X = T> struct SddmmEngine
         }
         if constexpr (Q8) sc[u] = act ? __ldg(bscale + (size_t)c * bstride) : 0.f;
       }
+      if constexpr (HL > 0) {
+        store_heads(d, col_ok, g, li, nst, jend - j0 - g, out + (ring.base + j0) * heads);
+      } else {
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+          float sdot = 0.f;
+#pragma unroll
+          for (int ch = 0; ch < CH; ch++) sdot += Vec16<X, VEC>::dot(d[u][ch], gq[ch]);
+          part[u] = sdot;
+        }
+        // lane li of group g gets the total of step li / (LPR/U); nnz t = u*G + g of the chunk goes to lane t
+        float tot = multi_reduce<U, LPR / 2>(part, li);
+        if constexpr (Q8) {  // the scale product, on the lane that holds the step's total
+          const int ul = li / (LPR / U);
+          float sb = sc[0];
+#pragma unroll
+          for (int u = 1; u < U; u++)
+            if (ul == u) sb = sc[u];
+          tot = __fmul_rn(__fmul_rn(scale, sb), tot);
+        }
+        const bool mine = lane < jend - j0;
+        const int src_lane = mine ? (lane % G) * LPR + (lane / G) * (LPR / U) : 0;
+        const float got = __shfl_sync(0xffffffffu, tot, src_lane);
+        if constexpr (Q8) {
+          if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got);
+        } else {
+          if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got * scale);
+        }
+      }
+    }
+  }
+
+  // HL > 0: the scores of one chunk (nst steps; lane group g is active in step u iff u * G < jrel) into outc, the
+  // chunk's first [H] row. Head h of a chunk-ch vector is (ch * LPR + li) / HL; the lane holding a (step, head)
+  // total stores it, so a step's G * H scores leave as one contiguous run.
+  int heads;
+  __device__ __forceinline__ void store_heads(const uint4 (&d)[U][CH], const bool (&col_ok)[CH], int g, int li,
+                                              int nst, int jrel, T* __restrict__ outc) {
+    const int hl = li & (HL - 1);
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) {
+      const int h = (ch * LPR + li) / HL;
+      float part[U];
 #pragma unroll
       for (int u = 0; u < U; u++) {
         float sdot = 0.f;
-#pragma unroll
-        for (int ch = 0; ch < CH; ch++) sdot += Vec16<X, VEC>::dot(d[u][ch], gq[ch]);
+        sdot += Vec16<X, VEC>::dot(d[u][ch], gq[ch]);
         part[u] = sdot;
       }
-      // lane li of group g gets the total of step li / (LPR/U); nnz t = u*G + g of the chunk goes to lane t
-      float tot = multi_reduce<U, LPR / 2>(part, li);
-      if constexpr (Q8) {  // the scale product, on the lane that holds the step's total
-        const int ul = li / (LPR / U);
-        float sb = sc[0];
+      if constexpr (U <= HL) {  // halving butterfly: lane hl of the head gets the total of step hl / (HL / U)
+        const float tot = multi_reduce<U, HL / 2>(part, hl);
+        const int u = hl / (HL / U);
+        if (hl % (HL / U) == 0 && col_ok[ch] && u < nst && u * G < jrel)
+          outc[(int64_t)(u * G + g) * heads + h] = Traits<T>::from_acc(tot * 1.f);
+      } else {  // fewer lanes per head than steps: every step reduced on its own
 #pragma unroll
-        for (int u = 1; u < U; u++)
-          if (ul == u) sb = sc[u];
-        tot = __fmul_rn(__fmul_rn(scale, sb), tot);
-      }
-      const bool mine = lane < jend - j0;
-      const int src_lane = mine ? (lane % G) * LPR + (lane / G) * (LPR / U) : 0;
-      const float got = __shfl_sync(0xffffffffu, tot, src_lane);
-      if constexpr (Q8) {
-        if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got);
-      } else {
-        if (mine) out[ring.base + j0 + lane] = Traits<T>::from_acc(got * scale);
+        for (int u = 0; u < U; u++) {
+          float t = part[u];
+#pragma unroll
+          for (int off = HL / 2; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
+          if (hl == 0 && col_ok[ch] && u < nst && u * G < jrel)
+            outc[(int64_t)(u * G + g) * heads + h] = Traits<T>::from_acc(t);
+        }
       }
     }
   }
 };
 
 // X = e4m3: gscale[row * gstride] is the row operand's scale, p.scale[col * p.scale_stride] the gathered row's
-template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T, int HL = 0>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__ out, const float* __restrict__ gscale,
                  uint32_t gstride) {
-  using Eng = SddmmEngine<T, LPR, CH, U, X>;
+  using Eng = SddmmEngine<T, LPR, CH, U, X, HL>;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -318,6 +359,7 @@ sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
       const int e = __shfl_sync(0xffffffffu, e_rel, rl);
       if (e == s) continue;
       Eng eng;
+      if constexpr (HL > 0) eng.heads = p.heads;
       eng.load_grad((const char*)grad + (r0 + rl) * (int64_t)row_bytes, col_ok, li);
       if constexpr (Eng::Q8) {
         const float scale = __ldg(gscale + (r0 + rl) * gstride);
@@ -331,11 +373,11 @@ sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
   }
 }
 
-template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T, int HL = 0>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__ out, const float* __restrict__ gscale,
                  uint32_t gstride) {
-  using Eng = SddmmEngine<T, LPR, CH, U, X>;
+  using Eng = SddmmEngine<T, LPR, CH, U, X, HL>;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -362,6 +404,7 @@ sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
     const int64_t base = S.start & ~(int64_t)31;
     ring.reset(base, S.end);
     Eng eng;
+    if constexpr (HL > 0) eng.heads = p.heads;
     eng.load_grad((const char*)grad + S.row_b * (int64_t)row_bytes, col_ok, li);
     if constexpr (Eng::Q8) {
       eng.run(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, li, pol, out,
@@ -378,11 +421,11 @@ sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
   }
 }
 
-template <typename T, int LPR, int CH, int U, int MINB, typename X = T>
+template <typename T, int LPR, int CH, int U, int MINB, typename X = T, int HL = 0>
 static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t st, const float* gscale = nullptr,
                         uint32_t gstride = 0) {
-  auto* kmain = sddmm_vec_kernel<T, LPR, CH, U, MINB, X>;
-  auto* kseg = sddmm_seg_kernel<T, LPR, CH, U, MINB, X>;
+  auto* kmain = sddmm_vec_kernel<T, LPR, CH, U, MINB, X, HL>;
+  auto* kseg = sddmm_seg_kernel<T, LPR, CH, U, MINB, X, HL>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
@@ -405,6 +448,59 @@ template <typename T> static int dispatch_sddmm(const SpmmParams& p, const void*
   if (vecs <= 16) return launch_sddmm<T, 16, 1, 4, 5>(p, grad, out, st);
   if (vecs <= 32) return launch_sddmm<T, 32, 1, 4, 4>(p, grad, out, st);
   return launch_sddmm<T, 32, 2, 4, 3>(p, grad, out, st);  // up to 64 vectors
+}
+
+// per-head scores (tsb200_sddmm_heads): vecs = H * HL vectors per row, HL lanes per head; the single-head
+// (LPR, CH, U) with one CTA/SM less (the per-head reduction and stores spill at the single-head occupancy)
+template <typename T, int HL> static int dispatch_sddmm_heads_lpr(const SpmmParams& p, const void* a, void* out,
+                                                                   cudaStream_t st) {
+  constexpr int VEC = 16 / sizeof(T);
+  const int64_t vecs = p.K / VEC;
+  if constexpr (HL <= 4) if (vecs <= 4) return launch_sddmm<T, 4, 1, 4, 4, T, HL>(p, a, out, st);
+  if constexpr (HL <= 8) if (vecs <= 8) return launch_sddmm<T, 8, 1, 4, 4, T, HL>(p, a, out, st);
+  if constexpr (HL <= 16) if (vecs <= 16) return launch_sddmm<T, 16, 1, 4, 4, T, HL>(p, a, out, st);
+  if (vecs <= 32) return launch_sddmm<T, 32, 1, 4, 3, T, HL>(p, a, out, st);
+  return launch_sddmm<T, 32, 2, 4, 2, T, HL>(p, a, out, st);  // up to 64 vectors
+}
+template <typename T> static int dispatch_sddmm_heads(const SpmmParams& p, int hl, const void* a, void* out,
+                                                      cudaStream_t st) {
+  switch (hl) {
+    case 1: return dispatch_sddmm_heads_lpr<T, 1>(p, a, out, st);
+    case 2: return dispatch_sddmm_heads_lpr<T, 2>(p, a, out, st);
+    case 4: return dispatch_sddmm_heads_lpr<T, 4>(p, a, out, st);
+    case 8: return dispatch_sddmm_heads_lpr<T, 8>(p, a, out, st);
+    case 16: return dispatch_sddmm_heads_lpr<T, 16>(p, a, out, st);
+    case 32: return dispatch_sddmm_heads_lpr<T, 32>(p, a, out, st);
+  }
+  return TSB200_ERR_UNSUPPORTED;
+}
+
+// generic per-head SDDMM: warp per CSR row, per (entry, head) the lanes stride over the D columns and the warp
+// reduces, as value_bw_generic_kernel does for one head
+template <typename T>
+__global__ void __launch_bounds__(256)
+sddmm_heads_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restrict__ col,
+                           const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ out, int64_t M,
+                           int64_t H, int64_t D) {
+  using acc_t = typename Traits<T>::acc_t;
+  const int lane = threadIdx.x & 31;
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t K = H * D;
+  for (int64_t m = wid; m < M; m += nw) {
+    const int64_t rs = rowptr[m], re = rowptr[m + 1];
+    for (int64_t e = rs; e < re; e++) {
+      const T* bp = b + col[e] * K;
+      for (int64_t h = 0; h < H; h++) {
+        acc_t s = (acc_t)0;
+        for (int64_t k = lane; k < D; k += 32)
+          s += Traits<T>::to_acc(a[m * K + h * D + k]) * Traits<T>::to_acc(bp[h * D + k]);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if (lane == 0) out[e * H + h] = Traits<T>::from_acc(s);
+      }
+    }
+  }
 }
 
 // e4m3 operands, output type T: a vector is 16 columns, so a K-column row is K / 16 vectors (K <= 2048)
@@ -663,6 +759,55 @@ extern "C" int tsb200_spmm_minmax_bw(const int64_t* col, const void* value, cons
     if (blocks > cap) blocks = cap;
     minmax_bw_kernel<T, A><<<(int)blocks, 256, 0, st>>>(col, (const T*)value, (const T*)mat, (const T*)grad_out,
                                                        arg_out, (A*)grad_value, (A*)grad_mat, B, M, N, K, E, lsl);
+    TSB_LAUNCH_CHECK();
+    return 0;
+  });
+}
+
+// ---- SDDMM with per-head scores (tsb200_sddmm_heads) ----------------------------------------------------------------
+// out[e, h] = <a[row_e, h, :], b[col_e, h, :]>. Row-wise kernels when D * sizeof(T) / 16 = HL is a power of two and
+// the row is at most 64 vectors with HL <= LPR; the generic kernel otherwise.
+extern "C" int tsb200_sddmm_heads(const int64_t* rowptr, const int64_t* col, const void* a, const void* b, void* out,
+                                  int64_t M, int64_t N, int64_t H, int64_t D, int64_t E, int dtype, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || H < 0 || D < 0 || E < 0) return TSB200_ERR_INVALID_ARG;
+  if (dtype != TSB200_F32 && dtype != TSB200_F64 && dtype != TSB200_F16 && dtype != TSB200_BF16)
+    return TSB200_ERR_UNSUPPORTED;
+  if (H > 0 && D > ((int64_t)1 << 40) / H) return TSB200_ERR_UNSUPPORTED;
+  if (E * H == 0) return 0;  // nothing to write
+  if (!out) return TSB200_ERR_INVALID_ARG;
+  const size_t es = dtype_size(dtype);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (D == 0) {  // every dot product is empty: +0
+    TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(E * H) * es, st));
+    return 0;
+  }
+  if (!rowptr || !col || !a || !b) return TSB200_ERR_INVALID_ARG;
+  const int64_t K = H * D;
+  const int64_t hl = (D * (int64_t)es) % 16 == 0 ? D * (int64_t)es / 16 : 0;
+  const int64_t vecs = hl * H;
+  const int64_t lpr = vecs <= 4 ? 4 : vecs <= 8 ? 8 : vecs <= 16 ? 16 : 32;
+  if (dtype != TSB200_F64 && hl > 0 && (hl & (hl - 1)) == 0 && hl <= lpr && vecs <= 64 &&
+      E < ((int64_t)1 << 31) - 64 && E * H < ((int64_t)1 << 40) && M < ((int64_t)1 << 32) &&
+      N < ((int64_t)1 << 32) && !((uintptr_t)a & 15) && !((uintptr_t)b & 15) && !((uintptr_t)col & 7) &&
+      !((uintptr_t)out % es) && workspace && !((uintptr_t)workspace & 255)) {
+    const WsLayout L = ws_layout(1, K, E, false, false);
+    if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+    SpmmParams p{rowptr, col, nullptr, b, nullptr, nullptr, 1, M, N, K, E};
+    p.heads = (int)H;
+    bind_ws(p, (char*)workspace, L, false);
+    switch (dtype) {
+      case TSB200_F32: return dispatch_sddmm_heads<float>(p, (int)hl, a, out, st);
+      case TSB200_F16: return dispatch_sddmm_heads<__half>(p, (int)hl, a, out, st);
+      case TSB200_BF16: return dispatch_sddmm_heads<__nv_bfloat16>(p, (int)hl, a, out, st);
+    }
+  }
+  return dispatch_float_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    int64_t blocks = (M + 7) / 8;
+    if (blocks > (int64_t)num_sms() * 32) blocks = (int64_t)num_sms() * 32;
+    sddmm_heads_generic_kernel<T><<<(int)blocks, 256, 0, st>>>(rowptr, col, (const T*)a, (const T*)b, (T*)out, M, H,
+                                                               D);
     TSB_LAUNCH_CHECK();
     return 0;
   });

@@ -70,6 +70,10 @@ struct SpmmParams {
   const uint8_t* res8;
   const float* res_scale;
   uint32_t res_stride;
+  // multi-head operands (tsb200_spmm_heads / tsb200_sddmm_heads, HEADS kernels only): K = heads * D, and the weight of
+  // column k of entry e is value[e * heads + k / D]. It fills the struct's tail padding, so the parameter offsets of
+  // every kernel that takes further arguments stay as they were.
+  int heads;
 };
 
 // ---- the deferral rule of the row-split kernels -------------------------------------------------

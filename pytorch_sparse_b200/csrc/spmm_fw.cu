@@ -33,9 +33,20 @@ namespace tsb {
 // compiler lays the stores out differently.
 __device__ __forceinline__ int64_t stored_arg(int a, int64_t E) { return a != 0x7fffffff ? (int64_t)a : E; }
 
+template <typename T> __device__ __forceinline__ typename Vec<T>::vraw load_vraw(const T* p);
+template <> __device__ __forceinline__ float load_vraw<float>(const float* p) { return __ldg(p); }
+template <> __device__ __forceinline__ unsigned short load_vraw<__nv_bfloat16>(const __nv_bfloat16* p) {
+  return __ldg(reinterpret_cast<const unsigned short*>(p));
+}
+template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __half* p) {
+  return __ldg(reinterpret_cast<const unsigned short*>(p));
+}
+
 // T = value / output type, X = dense-operand type: T itself, or __nv_fp8_e4m3 (tsb200_spmm_fw_fp8), in which case
 // every entry's weight is fl32(value * scale[col]) and a 16-byte gather carries 16 columns.
-template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct RowEngine {
+// HEADS (tsb200_spmm_heads, sum only): the value is [E, heads] and a 16-byte chunk lies inside one head, so the lane
+// weighs chunk ch of entry e by hval[e * heads + hcol[ch]], loaded next to the column word instead of the ring's value.
+template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEADS = false> struct RowEngine {
   using V = Vec<T>;
   static constexpr bool Q8 = !std::is_same<X, T>::value;
   static constexpr int VEC = Vec<X>::VEC;
@@ -47,6 +58,9 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
   int arg[ARG ? NA : 1];
   const float* scale;  // Q8 only
   uint32_t sstride;
+  const T* hval;       // HEADS only
+  int heads;
+  int hcol[HEADS ? CH : 1];
 
   __device__ __forceinline__ float acc_float(int i) const { return acc[i]; }
 
@@ -117,16 +131,20 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
       const int jabs0 = (int)ring.base + j0 + g;  // absolute nnz index of step 0 (E < 2^31)
       uint4 d[U][CH];
       VR v[U];
+      VR hv[HEADS ? U : 1][HEADS ? CH : 1];
       float sc[U];
       if (jend - j0 == U * G) {  // full chunk: every lane group has work in every step
 #pragma unroll
         for (int u = 0; u < U; u++) {
           const uint32_t c = pc[2 * u * G];
-          v[u] = pv[u * G];
+          if constexpr (!HEADS) v[u] = pv[u * G];
           const char* src = matb + (uint64_t)c * row_bytes;
 #pragma unroll
-          for (int ch = 0; ch < CH; ch++)
+          for (int ch = 0; ch < CH; ch++) {
             if (col_ok[ch]) d[u][ch] = ldg128_hint(src + ch * (LPR * 16), pol);
+            if constexpr (HEADS)
+              if (col_ok[ch]) hv[u][ch] = load_vraw<T>(hval + (int64_t)(jabs0 + u * G) * heads + hcol[ch]);
+          }
           if constexpr (Q8) sc[u] = row_scale(c);
         }
 #pragma unroll
@@ -134,7 +152,8 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
 #pragma unroll
           for (int ch = 0; ch < CH; ch++) {
             if (!col_ok[ch]) continue;
-            step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
+            if constexpr (HEADS) step(ch, hv[u][ch], 1.f, d[u][ch], jabs0 + u * G);
+            else step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
           }
         }
       } else {
@@ -146,11 +165,14 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
           if (u >= nst) break;
           act[u] = u * G < jrel;
           const uint32_t c = pc[2 * u * G];
-          v[u] = pv[u * G];
+          if constexpr (!HEADS) v[u] = pv[u * G];
           const char* src = matb + (uint64_t)c * row_bytes;
 #pragma unroll
-          for (int ch = 0; ch < CH; ch++)
+          for (int ch = 0; ch < CH; ch++) {
             if (act[u] && col_ok[ch]) d[u][ch] = ldg128_hint(src + ch * (LPR * 16), pol);
+            if constexpr (HEADS)
+              if (act[u] && col_ok[ch]) hv[u][ch] = load_vraw<T>(hval + (int64_t)(jabs0 + u * G) * heads + hcol[ch]);
+          }
           if constexpr (Q8) sc[u] = act[u] ? row_scale(c) : 0.f;
         }
 #pragma unroll
@@ -159,7 +181,8 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct Ro
 #pragma unroll
           for (int ch = 0; ch < CH; ch++) {
             if (!(act[u] && col_ok[ch])) continue;
-            step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
+            if constexpr (HEADS) step(ch, hv[u][ch], 1.f, d[u][ch], jabs0 + u * G);
+            else step(ch, v[u], Q8 ? sc[u] : 1.f, d[u][ch], jabs0 + u * G);
           }
         }
       }
@@ -472,14 +495,35 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
 };
 
 // min/max over an fp8 operand compare in fp32 (the packed engine multiplies two values of the storage type)
-template <typename T, int RED, int LPR, int CH, int U, typename X = T> struct EngineFor {
+template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEADS = false> struct EngineFor {
+  static_assert(!HEADS || (RED == R_SUM && std::is_same<X, T>::value), "per-head weights: sum over a T operand");
   using type = typename std::conditional<(RED != R_SUM && is_float16<T>::value && std::is_same<X, T>::value),
-                                         MinMax16Engine<T, RED, LPR, CH, U>, RowEngine<T, RED, LPR, CH, U, X>>::type;
+                                         MinMax16Engine<T, RED, LPR, CH, U>,
+                                         RowEngine<T, RED, LPR, CH, U, X, HEADS>>::type;
 };
 template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, const SpmmParams& p) {
   if constexpr (Eng::Q8) {
     eng.scale = p.scale;
     eng.sstride = p.scale_stride;
+  }
+}
+// HEADS: the head of each of this lane's chunks (chunk ch starts at column k0 + (ch * LPR + li) * VEC), computed once
+// per kernel by head_cols, and handed to every row's engine by set_heads
+template <bool HEADS, int LPR, int VEC, int CH>
+__device__ __forceinline__ void head_cols(int (&hcol)[HEADS ? CH : 1], const SpmmParams& p, int li) {
+  if constexpr (HEADS) {
+    const int D = (int)(p.K / p.heads);
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) hcol[ch] = (p.k0 + (ch * LPR + li) * VEC) / D;
+  }
+}
+template <bool HEADS, typename Eng, int NH>
+__device__ __forceinline__ void set_heads(Eng& eng, const SpmmParams& p, const int (&hcol)[NH]) {
+  if constexpr (HEADS) {
+    eng.hval = (decltype(eng.hval))p.value;
+    eng.heads = p.heads;
+#pragma unroll
+    for (int i = 0; i < NH; i++) eng.hcol[i] = hcol[i];
   }
 }
 
@@ -608,11 +652,12 @@ __device__ __forceinline__ void store_partial(const SpmmParams& p, const Eng& en
 }
 
 // QO: e4m3 result with per-row scales (RowEngine::store_row_q8) instead of T. RES: plus an e4m3 residual per row.
+// HEADS: per-head weights (tsb200_spmm_heads); the ring then streams the column words only.
 template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
-          bool QO = false, bool RES = false>
+          bool QO = false, bool RES = false, bool HEADS = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_vec_kernel(const SpmmParams p) {
-  using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
+  using Eng = typename EngineFor<T, RED, LPR, CH, U, X, HEADS>::type;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
@@ -623,20 +668,22 @@ spmm_vec_kernel(const SpmmParams p) {
   IndexRing<T> ring;
   ring.s_col = s_col[warp];
   ring.s_val = s_val[warp];
-  ring.has_val = p.value != nullptr;
-  if (!ring.has_val) {  // has_value=false: the ring's value half is a constant 1
+  ring.has_val = !HEADS && p.value != nullptr;
+  if (!HEADS && !ring.has_val) {  // has_value=false: the ring's value half is a constant 1
     using VR = typename Vec<T>::vraw;
     for (int i = lane; i < kRingAlloc; i += 32) reinterpret_cast<VR*>(s_val[warp])[i] = Vec<T>::one();
     __syncwarp();
   }
   ring.col = p.col;
-  ring.val = (const T*)p.value;
+  ring.val = HEADS ? nullptr : (const T*)p.value;
   ring.limit = p.E;
   const uint64_t pol = make_policy_evict_last();
 
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
+  int hcol[HEADS ? CH : 1];
+  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
   const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
   const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
 
@@ -687,6 +734,7 @@ spmm_vec_kernel(const SpmmParams p) {
       Eng eng;
       eng.init();
       set_scale(eng, p);
+      set_heads<HEADS>(eng, p, hcol);
       eng.accumulate(ring, s, e, matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
       if constexpr (QO) {
@@ -723,6 +771,7 @@ spmm_vec_kernel(const SpmmParams p) {
       Eng eng;
       eng.init();
       set_scale(eng, p);
+      set_heads<HEADS>(eng, p, hcol);
       eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
       if (S.slot < 0) {
@@ -765,21 +814,14 @@ spmm_vec_kernel(const SpmmParams p) {
 // reduction, per-row overhead amortised over G rows, U independent (index -> gather) chains in flight
 // per lane. Indices are read straight from global memory (lanes of a group broadcast one address,
 // consecutive nnz hit L1). Long rows / budget overflow still go to the segment queue.
-template <typename T> __device__ __forceinline__ typename Vec<T>::vraw load_vraw(const T* p);
-template <> __device__ __forceinline__ float load_vraw<float>(const float* p) { return __ldg(p); }
-template <> __device__ __forceinline__ unsigned short load_vraw<__nv_bfloat16>(const __nv_bfloat16* p) {
-  return __ldg(reinterpret_cast<const unsigned short*>(p));
-}
-template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __half* p) {
-  return __ldg(reinterpret_cast<const unsigned short*>(p));
-}
 
+// HEADS: the weight of entry j for this lane's chunk is val[j * heads + hcol], loaded in place of val[j].
 template <typename T, int RED, int LPR, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
-          bool QO = false, bool RES = false>
+          bool QO = false, bool RES = false, bool HEADS = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_gpr_kernel(const SpmmParams p) {
   using V = Vec<T>;
-  using Eng = typename EngineFor<T, RED, LPR, 1, U, X>::type;  // per-lane state + update + store of one row
+  using Eng = typename EngineFor<T, RED, LPR, 1, U, X, HEADS>::type;  // per-lane state + update + store of one row
   using VR = typename V::vraw;
   constexpr int VEC = Eng::VEC;
   constexpr bool Q8 = Eng::Q8;
@@ -792,6 +834,9 @@ spmm_gpr_kernel(const SpmmParams p) {
   const uint64_t pol = make_policy_evict_last();
   const T* __restrict__ val = (const T*)p.value;
   const bool has_val = val != nullptr;
+  int hcol[1];
+  head_cols<HEADS, LPR, VEC, 1>(hcol, p, li);
+  const int hstride = HEADS ? p.heads : 1;  // value elements per entry
 
   const int item_rows = 1 << p.item_shift;
   const int64_t nblk = (p.M + item_rows - 1) >> p.item_shift;
@@ -828,7 +873,7 @@ spmm_gpr_kernel(const SpmmParams p) {
     const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
     asm volatile("" : "+l"(matb));
     const int64_t* __restrict__ colb = p.col + base;
-    const T* __restrict__ valb = has_val ? val + base : nullptr;
+    const T* __restrict__ valb = has_val ? (HEADS ? val + base * hstride + hcol[0] : val + base) : nullptr;
     T* outb = (T*)p.out + (b * p.M + r0) * p.K + p.k0;
     int64_t* argb = p.arg_out ? p.arg_out + (b * p.M + r0) * p.K + p.k0 : nullptr;
     float* partb = ACC ? p.partial + (b * p.M + r0) * p.K + p.k0 : nullptr;
@@ -858,7 +903,11 @@ spmm_gpr_kernel(const SpmmParams p) {
         vn[u] = V::one();
         if (u < len) {
           cn[u] = (uint32_t)__ldg(colb + s + u);
-          if (has_val) vn[u] = load_vraw<T>(valb + s + u);
+          if constexpr (HEADS) {
+            if (col_ok) vn[u] = load_vraw<T>(valb + (int64_t)(s + u) * hstride);
+          } else {
+            if (has_val) vn[u] = load_vraw<T>(valb + s + u);
+          }
         }
       }
       for (int j0 = 0; j0 < maxlen; j0 += U) {
@@ -878,7 +927,11 @@ spmm_gpr_kernel(const SpmmParams p) {
           const int jn = j0 + U + u;
           if (jn < len) {
             cn[u] = (uint32_t)__ldg(colb + s + jn);
-            if (has_val) vn[u] = load_vraw<T>(valb + s + jn);
+            if constexpr (HEADS) {
+              if (col_ok) vn[u] = load_vraw<T>(valb + (int64_t)(s + jn) * hstride);
+            } else {
+              if (has_val) vn[u] = load_vraw<T>(valb + s + jn);
+            }
           }
         }
 #pragma unroll
@@ -908,10 +961,10 @@ spmm_gpr_kernel(const SpmmParams p) {
 
 // one warp per queued segment
 template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, typename X = T, bool QO = false,
-          bool RES = false>
+          bool RES = false, bool HEADS = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
 spmm_seg_kernel(const SpmmParams p) {
-  using Eng = typename EngineFor<T, RED, LPR, CH, U, X>::type;
+  using Eng = typename EngineFor<T, RED, LPR, CH, U, X, HEADS>::type;
   constexpr int VEC = Eng::VEC;
   __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
   __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
@@ -921,20 +974,22 @@ spmm_seg_kernel(const SpmmParams p) {
   IndexRing<T> ring;
   ring.s_col = s_col[warp];
   ring.s_val = s_val[warp];
-  ring.has_val = p.value != nullptr;
-  if (!ring.has_val) {  // has_value=false: the ring's value half is a constant 1
+  ring.has_val = !HEADS && p.value != nullptr;
+  if (!HEADS && !ring.has_val) {  // has_value=false: the ring's value half is a constant 1
     using VR = typename Vec<T>::vraw;
     for (int i = lane; i < kRingAlloc; i += 32) reinterpret_cast<VR*>(s_val[warp])[i] = Vec<T>::one();
     __syncwarp();
   }
   ring.col = p.col;
-  ring.val = (const T*)p.value;
+  ring.val = HEADS ? nullptr : (const T*)p.value;
   ring.limit = p.E;
   const uint64_t pol = make_policy_evict_last();
 
   bool col_ok[CH];
 #pragma unroll
   for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
+  int hcol[HEADS ? CH : 1];
+  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
   const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
   const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
 
@@ -950,6 +1005,7 @@ spmm_seg_kernel(const SpmmParams p) {
     Eng eng;
     eng.init();
     set_scale(eng, p);
+    set_heads<HEADS>(eng, p, hcol);
     eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
     eng.reduce_groups();
     if (g == 0) {
@@ -1114,15 +1170,15 @@ static void launch_combine(const SpmmParams& p, int kcols, cudaStream_t st) {
 }
 
 template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false,
-          typename X = T, bool QO = false, bool RES = false>
+          typename X = T, bool QO = false, bool RES = false, bool HEADS = false>
 static int launch_vec(SpmmParams p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(X);
   constexpr int kcols = LPR * CH * VEC;
   void (*kmain)(const SpmmParams);
-  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X, QO, RES>;
-  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X, QO, RES>;
+  if constexpr (GPR) kmain = spmm_gpr_kernel<T, RED, LPR, U, MINB, ACC, PLAN, X, QO, RES, HEADS>;
+  else kmain = spmm_vec_kernel<T, RED, LPR, CH, U, MINB, ACC, PLAN, X, QO, RES, HEADS>;
   constexpr int USEG = (U > LPR) ? LPR : U;  // the row engine needs U * (32 / LPR) <= 32
-  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO, RES>;
+  auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO, RES, HEADS>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
   const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
   p.item_shift = item_shift_for(p.M * p.B, grid_main);
@@ -1212,6 +1268,22 @@ static int dispatch_red_vec(SpmmParams p, int reduce, cudaStream_t st) {
     }
     return TSB200_ERR_INVALID_ARG;
   }
+}
+
+// per-head weights (tsb200_spmm_heads): the sum kernels' shapes; (U, CTAs/SM) as for one head unless the weight
+// registers spill there (ptxas table in DESIGN §3.1)
+template <typename T, bool PLAN>
+static int dispatch_heads(const SpmmParams& p, cudaStream_t st) {
+  constexpr int VEC = 16 / sizeof(T);
+  const int64_t vecs = p.K / VEC;
+  if (vecs <= 1) return launch_vec<T, R_SUM, false, 1, 1, 4, 4, true, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 2) return launch_vec<T, R_SUM, false, 2, 1, 4, 4, true, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 4) return launch_vec<T, R_SUM, false, 4, 1, 4, 4, true, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 8) return launch_vec<T, R_SUM, false, 8, 1, 4, 4, true, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 16) return launch_vec<T, R_SUM, false, 16, 1, 6, 2, false, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 32) return launch_vec<T, R_SUM, false, 32, 1, 4, 4, false, PLAN, T, false, false, true>(p, st);
+  if (vecs <= 64) return launch_vec<T, R_SUM, false, 32, 2, 4, 2, false, PLAN, T, false, false, true>(p, st);
+  return launch_vec<T, R_SUM, false, 32, 4, 2, 2, false, PLAN, T, false, false, true>(p, st);
 }
 
 // ---- plan: the segment list of a matrix, built once (tsb200_spmm_plan) -----------------------------------------
@@ -1319,6 +1391,34 @@ static int bind_plan(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t
   p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
   p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
   return 0;
+}
+
+// generic per-head SpMM (tsb200_spmm_heads off the vector path): warp per row, lane per column k of the H * D, the
+// entries summed in order with one rounding per product and per sum, as spmm_generic_kernel does
+template <typename T>
+__global__ void __launch_bounds__(256)
+spmm_heads_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restrict__ col,
+                          const T* __restrict__ value, const T* __restrict__ mat, T* __restrict__ out, int64_t M,
+                          int64_t H, int64_t D) {
+  using acc_t = typename Traits<T>::acc_t;
+  const int64_t K = H * D;
+  const int lane = threadIdx.x & 31;
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t m = wid; m < M; m += nw) {
+    const int64_t rs = rowptr[m], re = rowptr[m + 1];
+    for (int64_t k = lane; k < K; k += 32) {
+      const int64_t h = k / D;
+      acc_t a = (acc_t)0;
+      for (int64_t e = rs; e < re; e++) {
+        const acc_t mv = Traits<T>::to_acc(mat[col[e] * K + k]);
+        const acc_t vv = Traits<T>::to_acc(value[e * H + h]);
+        if constexpr (std::is_same<acc_t, double>::value) a = __dadd_rn(a, __dmul_rn(vv, mv));
+        else a = __fadd_rn(a, __fmul_rn(vv, mv));
+      }
+      out[m * K + k] = Traits<T>::from_acc(a);
+    }
+  }
 }
 
 template <typename T, int RED>
@@ -1635,4 +1735,62 @@ extern "C" int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col,
   return spmm_fw_fp8_impl<false>(rowptr, col, value, mat, scale, scale_stride, out, nullptr, arg_out, M, N, K, E,
                                  out_dtype, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes,
                                  stream, (const uint8_t*)res8, res_scale, res_scale_stride);
+}
+
+// ---- SpMM with per-head weights (tsb200_spmm_heads) -------------------------------------------------------------
+// The sum kernels with HEADS = true over x [N, H * D]; with value == NULL every weight is 1 and the product is the
+// plain sum (tsb200_spmm_fw / tsb200_spmm_fw_planned over K = H * D columns).
+extern "C" int tsb200_spmm_heads(const int64_t* rowptr, const int64_t* col, const void* value, const void* x, void* out,
+                                 int64_t M, int64_t N, int64_t H, int64_t D, int64_t E, int dtype, const void* plan,
+                                 size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || H < 0 || D < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
+  if (dtype != TSB200_F32 && dtype != TSB200_F64 && dtype != TSB200_F16 && dtype != TSB200_BF16)
+    return TSB200_ERR_UNSUPPORTED;
+  if (H > 0 && D > ((int64_t)1 << 40) / H) return TSB200_ERR_UNSUPPORTED;
+  const int64_t K = H * D;
+  if (M * K == 0) return 0;  // nothing to write
+  if (!rowptr || !out) return TSB200_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (E == 0) {  // every row is empty: +0
+    TSB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)(M * K) * dtype_size(dtype), st));
+    return 0;
+  }
+  if (!col || !x) return TSB200_ERR_INVALID_ARG;
+  if (!value) {
+    if (plan) return tsb200_spmm_fw_planned(rowptr, col, nullptr, x, out, nullptr, M, N, K, E, dtype, TSB200_SUM, plan,
+                                            plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, stream);
+    return tsb200_spmm_fw(rowptr, col, nullptr, x, out, nullptr, 1, M, N, K, E, dtype, TSB200_SUM, workspace,
+                          workspace_bytes, stream);
+  }
+  const size_t es = dtype_size(dtype);
+  if ((D * (int64_t)es) % 16 == 0 && vec_eligible(dtype, K, E, N, value, x, out, col, nullptr) &&
+      H * E < ((int64_t)1 << 31)) {
+    SpmmParams p{rowptr, col, value, x, out, nullptr, 1, M, N, K, E};
+    p.heads = (int)H;
+    if (plan) {
+      if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, false))
+        return rc;
+    } else {
+      const WsLayout L = ws_layout(1, K, E, false);
+      if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+      if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
+      bind_ws(p, (char*)workspace, L, false);
+    }
+    switch (dtype) {
+      case TSB200_F32: return plan ? dispatch_heads<float, true>(p, st) : dispatch_heads<float, false>(p, st);
+      case TSB200_F16: return plan ? dispatch_heads<__half, true>(p, st) : dispatch_heads<__half, false>(p, st);
+      case TSB200_BF16:
+        return plan ? dispatch_heads<__nv_bfloat16, true>(p, st) : dispatch_heads<__nv_bfloat16, false>(p, st);
+    }
+  }
+  return dispatch_float_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    int64_t blocks = (M + 7) / 8;
+    if (blocks > (int64_t)num_sms() * 64) blocks = (int64_t)num_sms() * 64;
+    spmm_heads_generic_kernel<T><<<(int)blocks, 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)x, (T*)out, M,
+                                                              H, D);
+    TSB_LAUNCH_CHECK();
+    return 0;
+  });
 }

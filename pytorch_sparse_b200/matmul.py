@@ -180,6 +180,49 @@ def sddmm_fp8(src: SparseTensor, a8: Tensor, a_scale: Tensor, b8: Tensor, b_scal
     return torch.ops.tsb200.sddmm_fp8(rowptr, col, a8, a_scale, b8, b_scale, out_dtype)
 
 
+def spmm_heads(src: SparseTensor, x: Tensor) -> Tensor:
+    """Multi-head message passing: `out[m, h] = sum_e value[e, h] * x[col_e, h]` over the entries of row m, for `x`
+    [N, H, D] and a value of `src` of shape [E, H] (or none: every weight 1), `out` [M, H, D], without an E x H*D
+    temporary. The value is cast to x's dtype (bf16, f16, f32, f64); fp32 accumulation (fp64 for fp64), one rounding.
+    Differentiable in the value (an `sddmm_heads`) and in `x` (an `spmm_heads` on the cached CSC view). With H = 1 the
+    result is `spmm`'s, bit for bit."""
+    rowptr, col, value = src.csr()
+    st = src.storage
+    N = src.sparse_size(1)
+    if x.dim() == 3 and x.size(0) != N:
+        raise RuntimeError("spmm_heads: x must have " + str(N) + " rows (the sparse sizes), got " + str(x.size(0)))
+    row, colptr, csr2csc = st._row, st._colptr, st._csr2csc
+    row_csc: Optional[Tensor] = None
+    if value is not None:
+        value = value.to(x.dtype)
+    if x.requires_grad:     # grad_x = A^T @ grad_out per head runs on the CSC view
+        row = st.row()
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.spmm_heads(row, rowptr, col, value, colptr, csr2csc, x, row_csc)
+
+
+def sddmm_heads(src: SparseTensor, a: Tensor, b: Tensor) -> Tensor:
+    """Multi-head edge scores `s[e, h] = <a[row_e, h], b[col_e, h]>` for `a` [M, H, D] and `b` [N, H, D], `s` [E, H]
+    in CSR order, without an E x H*D temporary; dtypes and accumulation as `sddmm`, whose result it is for H = 1.
+    `src`'s values are ignored. Differentiable in `a` and `b` (`spmm_heads` on the CSR and the cached CSC view)."""
+    rowptr, col, _ = src.csr()
+    st = src.storage
+    M, N = src.sparse_sizes()
+    if a.dim() == 3 and b.dim() == 3 and (a.size(0) != M or b.size(0) != N):
+        raise RuntimeError("sddmm_heads: a must have " + str(M) + " rows and b " + str(N) + " rows (the sparse sizes), "
+                           "got " + str(a.size(0)) + " and " + str(b.size(0)))
+    row = st.row()
+    colptr, csr2csc = st._colptr, st._csr2csc
+    row_csc: Optional[Tensor] = None
+    if b.requires_grad:     # grad_b = A(g)^T @ a per head runs on the CSC view
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.sddmm_heads(row, rowptr, col, colptr, csr2csc, row_csc, a, b)
+
+
 def spspmm_sum(src: SparseTensor, other: SparseTensor) -> SparseTensor:
     M, Kd = src.sparse_sizes()
     Kb, N = other.sparse_sizes()
@@ -241,6 +284,8 @@ SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum", residual=Non
 SparseTensor.sddmm = lambda self, a, b: sddmm(self, a, b)
 SparseTensor.sddmm_fp8 = lambda self, a8, a_scale, b8, b_scale, out_dtype=torch.float32: sddmm_fp8(
     self, a8, a_scale, b8, b_scale, out_dtype)
+SparseTensor.spmm_heads = lambda self, x: spmm_heads(self, x)
+SparseTensor.sddmm_heads = lambda self, a, b: sddmm_heads(self, a, b)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)
 SparseTensor.__matmul__ = lambda self, other: matmul(self, other, "sum")

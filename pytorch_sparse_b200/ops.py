@@ -1094,6 +1094,163 @@ def sddmm(row: Tensor, rowptr: Tensor, col: Tensor, colptr: Optional[Tensor], cs
     return SDDMM.apply(row, rowptr, col, colptr, csr2csc, row_csc, a, b)
 
 
+# --------------------------------------------------------------------------------------------------
+# Multi-head SpMM / SDDMM: one weight per entry and head over [rows, H, D] operands
+# --------------------------------------------------------------------------------------------------
+def _heads_dtype(what: str, t: Tensor) -> None:
+    if not t.dtype.is_floating_point or t.dtype not in _DTYPES:
+        raise RuntimeError(f'"{what}" not implemented for \'{t.dtype}\'')
+
+
+def _spmm_heads_check(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x: Tensor,
+                      colptr: Optional[Tensor]) -> None:
+    for t, n in ((rowptr, "rowptr"), (col, "col"), (x, "x")):
+        _check_cuda(t, n)
+    if value is not None:
+        _check_cuda(value, "value")
+    if x.dim() != 3:
+        raise RuntimeError(f"spmm_heads: x must be 3-D [N, H, D], got {x.dim()}-D")
+    _heads_dtype("spmm_heads", x)
+    E, H = col.numel(), x.size(1)
+    if value is not None:
+        if value.dim() != 2 or value.size(0) != E or value.size(1) != H:
+            raise RuntimeError(f"spmm_heads: value must be [E, H] = [{E}, {H}], got {list(value.shape)}")
+        if value.dtype != x.dtype:
+            raise RuntimeError(f"spmm_heads: value and x must have the same dtype, got {value.dtype} and {x.dtype}")
+    if colptr is not None and colptr.numel() - 1 != x.size(0):
+        raise RuntimeError(f"spmm_heads: x must have {colptr.numel() - 1} rows (the matrix's columns), got {x.size(0)}")
+
+
+def _sddmm_heads_check(rowptr: Tensor, col: Tensor, a: Tensor, b: Tensor, colptr: Optional[Tensor]) -> None:
+    for t, n in ((rowptr, "rowptr"), (col, "col"), (a, "a"), (b, "b")):
+        _check_cuda(t, n)
+    for t, n in ((a, "a"), (b, "b")):
+        if t.dim() != 3:
+            raise RuntimeError(f"sddmm_heads: {n} must be 3-D [rows, H, D], got {t.dim()}-D")
+    _heads_dtype("sddmm_heads", a)
+    if b.dtype != a.dtype:
+        raise RuntimeError(f"sddmm_heads: a and b must have the same dtype, got {a.dtype} and {b.dtype}")
+    M = rowptr.numel() - 1
+    if a.size(0) != M or a.shape[1:] != b.shape[1:]:
+        raise RuntimeError(f"sddmm_heads: a must be [M, H, D] = [{M}, {b.size(1)}, {b.size(2)}] for b of shape "
+                           f"{list(b.shape)}, got {list(a.shape)}")
+    if colptr is not None and colptr.numel() - 1 != b.size(0):
+        raise RuntimeError(f"sddmm_heads: b must have {colptr.numel() - 1} rows (the matrix's columns), got {b.size(0)}")
+
+
+def _spmm_heads_fw(rowptr: Tensor, col: Tensor, value: Optional[Tensor], x: Tensor) -> Tensor:
+    """out [M, H, D] = per head h, sum over row m's entries of value[e, h] * x[col_e, h] (tsb200_spmm_heads); a
+    plannable product uses the plan cached for `rowptr`, like `spmm_fw`."""
+    rowptr, col, x = _i64(rowptr, "rowptr"), _i64(col, "col"), x.contiguous()
+    if value is not None:
+        value = value.contiguous()
+    M, (N, H, D), E = rowptr.numel() - 1, x.shape, col.numel()
+    dev = x.device
+    out = torch.empty((M, H, D), dtype=x.dtype, device=dev)
+    if out.numel() == 0:
+        return out
+    dt = _dtype_code(x.dtype)
+    with _on_device(dev):
+        plannable = E > 0 and dt in (0, 2, 3) and (D * x.element_size()) % 16 == 0
+        pl, ws, nws = _plan_workspace(None, plannable, rowptr, 1, M, H * D, E, dt, 0, dev)
+        check(lib.tsb200_spmm_heads(_p(rowptr), _p(col), _p(value), _p(x), _p(out), M, N, H, D, E, dt, *pl,
+                                    _p(ws), nws, _stream(dev)), "tsb200_spmm_heads")
+    return out
+
+
+def _sddmm_heads_fw(rowptr: Tensor, col: Tensor, a: Tensor, b: Tensor) -> Tensor:
+    """s [E, H] = per head h, <a[row_e, h], b[col_e, h]> in CSR order (tsb200_sddmm_heads)."""
+    rowptr, col, a, b = _i64(rowptr, "rowptr"), _i64(col, "col"), a.contiguous(), b.contiguous()
+    M, (N, H, D), E = rowptr.numel() - 1, b.shape, col.numel()
+    dev = a.device
+    out = torch.empty((E, H), dtype=a.dtype, device=dev)
+    if out.numel() == 0:
+        return out
+    dt = _dtype_code(a.dtype)
+    with _on_device(dev):
+        nws = lib.tsb200_spmm_value_bw_workspace_bytes(1, M, H * D, E, dt)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_sddmm_heads(_p(rowptr), _p(col), _p(a), _p(b), _p(out), M, N, H, D, E, dt, _p(ws), nws,
+                                     _stream(dev)), "tsb200_sddmm_heads")
+    return out
+
+
+class SPMMHeads(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, row, rowptr, col, value, colptr, csr2csc, x, row_csc=None):
+        has_value = value is not None
+        need_x = ctx.needs_input_grad[6]
+        if need_x:
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+            if row_csc is None:
+                _assert_present(row, "row")
+        out = _spmm_heads_fw(rowptr, col, value, x)
+        ctx.has_value = has_value
+        ctx.save_for_backward(row if need_x else None, rowptr, col, value, colptr if need_x else None,
+                              csr2csc if need_x else None, x if has_value and ctx.needs_input_grad[3] else None,
+                              row_csc if need_x else None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row, rowptr, col, value, colptr, csr2csc, x, row_csc = ctx.saved_tensors
+        grad_value = grad_x = None
+        if ctx.has_value and ctx.needs_input_grad[3]:     # d value[e, h] = <g[row_e, h], x[col_e, h]>
+            grad_value = _sddmm_heads_fw(rowptr, col, grad_out, x)
+        if ctx.needs_input_grad[6]:     # d x = A^T(value) @ g per head, on the CSC view
+            if row_csc is None:
+                row_csc = row.index_select(0, csr2csc)
+            v = value.index_select(0, csr2csc) if ctx.has_value else None
+            grad_x = _spmm_heads_fw(colptr, row_csc, v, grad_out)
+        return None, None, None, grad_value, None, None, grad_x, None
+
+
+class SDDMMHeads(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, row, rowptr, col, colptr, csr2csc, row_csc, a, b):
+        need_a, need_b = ctx.needs_input_grad[6], ctx.needs_input_grad[7]
+        if need_b:
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+        out = _sddmm_heads_fw(rowptr, col, a, b)
+        ctx.save_for_backward(row if need_b else None, rowptr if need_a else None, col if need_a else None,
+                              colptr if need_b else None, csr2csc if need_b else None,
+                              row_csc if need_b else None, a if need_b else None, b if need_a else None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row, rowptr, col, colptr, csr2csc, row_csc, a, b = ctx.saved_tensors
+        grad_a = grad_b = None
+        if ctx.needs_input_grad[6]:     # grad_a = A(g) @ b per head, on the CSR view
+            grad_a = _spmm_heads_fw(rowptr, col, grad_out, b)
+        if ctx.needs_input_grad[7]:     # grad_b = A(g)^T @ a per head, on the CSC view
+            if row_csc is None:
+                row_csc = row.index_select(0, csr2csc)
+            grad_b = _spmm_heads_fw(colptr, row_csc, grad_out.index_select(0, csr2csc), a)
+        return None, None, None, None, None, None, grad_a, grad_b
+
+
+def spmm_heads(row: Optional[Tensor], rowptr: Tensor, col: Tensor, value: Optional[Tensor], colptr: Optional[Tensor],
+               csr2csc: Optional[Tensor], x: Tensor, row_csc: Optional[Tensor] = None) -> Tensor:
+    """`out[m, h] = sum_{e in row m} value[e, h] * x[col_e, h]` for `x` [N, H, D] and `value` [E, H] (None: all ones),
+    `out` [M, H, D]; bf16 / f16 / f32 / f64 with fp32 accumulation (fp64 for fp64) and one rounding. Differentiable in
+    `value` (`sddmm_heads(g, x)`) and `x` (an `spmm_heads` on the CSC view, which needs `colptr`, `csr2csc` and `row`
+    or the cached `row_csc = row[csr2csc]`)."""
+    _spmm_heads_check(rowptr, col, value, x, colptr)
+    return SPMMHeads.apply(row, rowptr, col, value, colptr, csr2csc, x, row_csc)
+
+
+def sddmm_heads(row: Tensor, rowptr: Tensor, col: Tensor, colptr: Optional[Tensor], csr2csc: Optional[Tensor],
+                row_csc: Optional[Tensor], a: Tensor, b: Tensor) -> Tensor:
+    """`s[e, h] = <a[row_e, h], b[col_e, h]>` for `a` [M, H, D] and `b` [N, H, D], `s` [E, H] in CSR order; dtypes and
+    accumulation as `sddmm`. Differentiable in `a` (an `spmm_heads` with values g on the CSR view) and `b` (one on the
+    CSC view, which needs `colptr`, `csr2csc` and optionally the cached `row_csc`)."""
+    _sddmm_heads_check(rowptr, col, a, b, colptr)
+    return SDDMMHeads.apply(row, rowptr, col, colptr, csr2csc, row_csc, a, b)
+
+
 FP8_SDDMM_MAX_K = 2048
 
 

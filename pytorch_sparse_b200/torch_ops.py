@@ -3,7 +3,7 @@
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
     torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant,
-                      quantize_fp8, sddmm, sddmm_fp8}  (own additions)
+                      quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -55,6 +55,11 @@ _EXTRA_SCHEMAS = {
              "Tensor b) -> Tensor",
     "sddmm_fp8": "(Tensor rowptr, Tensor col, Tensor a8, Tensor a_scale, Tensor b8, Tensor b_scale, "
                  "ScalarType out_dtype) -> Tensor",
+    # multi-head: value [E, H] over x [N, H, D]; scores [E, H] of a [M, H, D] and b [N, H, D]
+    "spmm_heads": "(Tensor? row, Tensor rowptr, Tensor col, Tensor? value, Tensor? colptr, Tensor? csr2csc, "
+                  "Tensor x, Tensor? row_csc) -> Tensor",
+    "sddmm_heads": "(Tensor row, Tensor rowptr, Tensor col, Tensor? colptr, Tensor? csr2csc, Tensor? row_csc, "
+                   "Tensor a, Tensor b) -> Tensor",
 }
 
 
@@ -75,6 +80,7 @@ _EXTRA_IMPLS = {
         ops.spmm_fw_fp8_quant(rowptr, col, value, x8, scale, reduce, residual=residual, residual_scale=residual_scale),
     "quantize_fp8": ops.quantize_fp8,
     "sddmm": ops.sddmm, "sddmm_fp8": ops.sddmm_fp8,
+    "spmm_heads": ops.spmm_heads, "sddmm_heads": ops.sddmm_heads,
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -303,12 +303,7 @@ sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
   const int g = lane / LPR, li = lane % LPR;
 
   IndexRing<T> ring;
-  ring.s_col = s_col[warp];
-  ring.s_val = nullptr;
-  ring.has_val = false;
-  ring.col = p.col;
-  ring.val = nullptr;
-  ring.limit = p.E;
+  ring.template bind<false>(p, s_col[warp], nullptr, lane);
   const uint64_t pol = make_policy_evict_last();
 
   bool col_ok[CH];
@@ -320,13 +315,9 @@ sddmm_vec_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
 
   const int item_rows = 1 << p.item_shift;
   const int64_t n_items = (p.M + item_rows - 1) >> p.item_shift;
-  unsigned int item = 0;
-  if (lane == 0) item = atomicAdd(&p.counters[0], 1u);
-  item = __shfl_sync(0xffffffffu, item, 0);
-
+  unsigned int item = __shfl_sync(0xffffffffu, take_ticket(&p.counters[0], lane), 0);
   while ((int64_t)item < n_items) {
-    unsigned int next_item = 0;
-    if (lane == 0) next_item = atomicAdd(&p.counters[0], 1u);
+    const unsigned int next_item = take_ticket(&p.counters[0], lane);
     const int64_t r0 = (int64_t)item << p.item_shift;
     const int nrows = (int)min((int64_t)item_rows, p.M - r0);
     const int64_t rp0 = __ldg(p.rowptr + r0 + min(lane, nrows));
@@ -383,12 +374,7 @@ sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane / LPR, li = lane % LPR;
   IndexRing<T> ring;
-  ring.s_col = s_col[warp];
-  ring.s_val = nullptr;
-  ring.has_val = false;
-  ring.col = p.col;
-  ring.val = nullptr;
-  ring.limit = p.E;
+  ring.template bind<false>(p, s_col[warp], nullptr, lane);
   const uint64_t pol = make_policy_evict_last();
   bool col_ok[CH];
 #pragma unroll

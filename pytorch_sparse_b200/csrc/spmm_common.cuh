@@ -92,7 +92,16 @@ __device__ __forceinline__ bool defer_row(int deg, int lane) {
   return (deg > 0) && (is_long || cum > kItemCap);
 }
 
+// Lane 0's ticket from the counter c (0 on the other lanes): the work items, and the planned drain's segments, of the
+// row-split kernels are handed out this way.
+__device__ __forceinline__ unsigned int take_ticket(unsigned int* c, int lane) {
+  unsigned int t = 0;
+  if (lane == 0) t = atomicAdd(c, 1u);
+  return t;
+}
+
 // ---- per-warp streaming index ring ------------------------------------------------------------
+template <typename T> struct Vec;
 template <typename T> struct IndexRing {
   bool has_val;
   int64_t* s_col;
@@ -104,6 +113,25 @@ template <typename T> struct IndexRing {
   int issued_w;   // last window issued
   int ready_w;    // windows <= ready_w are complete and visible to the whole warp
 
+  // bind to this warp's shared arrays and to the index stream of p (entries [0, p.E)). VALUES: p.value streams next to
+  // the column words, or, when there is none, the value half holds a constant 1 (filled here, once). Without VALUES
+  // (the SDDMM, per-head weights) only the column words stream.
+  template <bool VALUES>
+  __device__ __forceinline__ void bind(const SpmmParams& p, int64_t* s_col_, T* s_val_, int lane) {
+    s_col = s_col_;
+    s_val = s_val_;
+    has_val = VALUES && p.value != nullptr;
+    if constexpr (VALUES) {
+      if (!has_val) {
+        using VR = typename Vec<T>::vraw;
+        for (int i = lane; i < kRingAlloc; i += 32) reinterpret_cast<VR*>(s_val)[i] = Vec<T>::one();
+        __syncwarp();
+      }
+    }
+    col = p.col;
+    val = VALUES ? (const T*)p.value : nullptr;
+    limit = p.E;
+  }
   // start streaming a new nnz range [.., limit_): copies still in flight from the previous range
   // (its last prefetched windows) must land before their slots are reused.
   __device__ __forceinline__ void reset(int64_t base_, int64_t limit_) {

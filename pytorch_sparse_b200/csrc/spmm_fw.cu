@@ -32,6 +32,17 @@ namespace tsb {
 // E. A row store passes E itself for an empty row (`count > 0 ? stored_arg(..) : E`); with that test in here the
 // compiler lays the stores out differently.
 __device__ __forceinline__ int64_t stored_arg(int a, int64_t E) { return a != 0x7fffffff ? (int64_t)a : E; }
+// the VEC arg slots of one chunk of a row of degree count, as longlong2 pairs streamed to arg_row (every row store)
+template <int VEC>
+__device__ __forceinline__ void store_args(int64_t* __restrict__ arg_row, const int* arg, int64_t count, int64_t E) {
+#pragma unroll
+  for (int i = 0; i < VEC; i += 2) {
+    longlong2 a2;
+    a2.x = count > 0 ? stored_arg(arg[i], E) : E;
+    a2.y = count > 0 ? stored_arg(arg[i + 1], E) : E;
+    stg128_stream(arg_row + i, *reinterpret_cast<uint4*>(&a2));
+  }
+}
 
 template <typename T> __device__ __forceinline__ typename Vec<T>::vraw load_vraw(const T* p);
 template <> __device__ __forceinline__ float load_vraw<float>(const float* p) { return __ldg(p); }
@@ -248,15 +259,7 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEAD
       }
 #pragma unroll
       for (int i = 0; i < VEC; i += V::VEC) stg128_stream(out_row + koff + i, V::pack(f + i));  // 2-4 stores for Q8
-      if (ARG) {
-#pragma unroll
-        for (int i = 0; i < VEC; i += 2) {
-          longlong2 a2;
-          a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
-          a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
-          stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
-        }
-      }
+      if (ARG) store_args<VEC>(arg_row + koff, &arg[ch * VEC], count, E);
     }
   }
 
@@ -298,15 +301,7 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEAD
       if (!col_ok[ch]) continue;
       const int koff = (ch * LPR + li) * VEC;
       stg128_stream(out_row + koff, e4m3_pack16(&acc[ch * VEC], s));
-      if (ARG) {
-#pragma unroll
-        for (int i = 0; i < VEC; i += 2) {
-          longlong2 a2;
-          a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
-          a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
-          stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
-        }
-      }
+      if (ARG) store_args<VEC>(arg_row + koff, &arg[ch * VEC], count, E);
     }
     if (li == 0) *scale_out = s;
   }
@@ -483,13 +478,7 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
       uint4 o = make_uint4(pacc[ch * 4], pacc[ch * 4 + 1], pacc[ch * 4 + 2], pacc[ch * 4 + 3]);
       if (count == 0) o = make_uint4(0, 0, 0, 0);
       stg128_stream(out_row + koff, o);
-#pragma unroll
-      for (int i = 0; i < VEC; i += 2) {
-        longlong2 a2;
-        a2.x = count > 0 ? stored_arg(arg[ch * VEC + i], E) : E;
-        a2.y = count > 0 ? stored_arg(arg[ch * VEC + i + 1], E) : E;
-        stg128_stream(arg_row + koff + i, *reinterpret_cast<uint4*>(&a2));
-      }
+      store_args<VEC>(arg_row + koff, &arg[ch * VEC], count, E);
     }
   }
 };
@@ -651,6 +640,105 @@ __device__ __forceinline__ void store_partial(const SpmmParams& p, const Eng& en
   }
 }
 
+// Where the final stores of rows r0 + rl of batch b go (T result: `out`, the ACC partial and arg_out, at column k0;
+// QO: an e4m3 result, B == 1, one column tile). The two main kernels make one per work item, next to the gather base.
+// store() is their final row store: the engine's store_row, or store_row_q8 for QO, called by the lanes that hold the
+// row. The segment kernel and the planned drain store a whole-row segment with their own copy of the call: through
+// RowOut the compiler orders their instructions differently (the e4m3-result min/max ones need more registers).
+template <typename T, bool ACC, bool QO, bool RES> struct RowOut {
+  T* outb;
+  int64_t* argb;
+  float* partb;
+  int64_t r0;
+
+  __device__ __forceinline__ RowOut(const SpmmParams& p, int64_t b, int64_t r0_) : r0(r0_) {
+    outb = (T*)p.out + (b * p.M + r0) * p.K + p.k0;
+    argb = p.arg_out ? p.arg_out + (b * p.M + r0) * p.K + p.k0 : nullptr;
+    partb = ACC ? p.partial + (b * p.M + r0) * p.K + p.k0 : nullptr;
+  }
+  template <typename Eng, int CH>
+  __device__ __forceinline__ void store(Eng& eng, const SpmmParams& p, int rl, int64_t count,
+                                        const bool (&col_ok)[CH], int li) const {
+    if constexpr (QO)
+      eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
+                                     argb ? argb + (int64_t)rl * p.K : nullptr, count, p.E, col_ok, li, p.mean != 0,
+                                     RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
+    else
+      eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, count, p.E,
+                                  col_ok, li, p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr,
+                                  ACC ? p.acc_mode : 0, RES ? res_row(p, r0 + rl) : nullptr,
+                                  RES ? res_scale(p, r0 + rl) : 0.f);
+  }
+};
+
+// ---- the front of a main kernel's work items ------------------------------------------------------
+// A warp takes tickets from p.counters[0]; start() takes the next one as an item starts, so that the atomic's latency
+// hides behind the item. Ticket t is row block t % nblk of batch b = t / nblk: rows [r0, r0 + nrows), 2^item_shift of
+// them but fewer at the end. Lane l holds the nnz range [rp0, rp1) of row r0 + l (lanes >= nrows: the item's end).
+//   for (WorkItem it(p, lane); it.start(p, lane); it.advance()) { ... }
+struct WorkItem {
+  int item_rows;
+  int64_t nblk, n_items;
+  unsigned int ticket, next_ticket;
+  int64_t b, r0, rp0, rp1;
+  int nrows;
+
+  __device__ __forceinline__ WorkItem(const SpmmParams& p, int lane) {
+    item_rows = 1 << p.item_shift;
+    nblk = (p.M + item_rows - 1) >> p.item_shift;
+    n_items = nblk * p.B;
+    ticket = __shfl_sync(0xffffffffu, take_ticket(&p.counters[0], lane), 0);
+  }
+  __device__ __forceinline__ bool start(const SpmmParams& p, int lane) {
+    if ((int64_t)ticket >= n_items) return false;
+    next_ticket = take_ticket(&p.counters[0], lane);
+    b = ticket / nblk;
+    r0 = (ticket - b * nblk) << p.item_shift;
+    nrows = (int)min((int64_t)item_rows, p.M - r0);
+    rp0 = __ldg(p.rowptr + r0 + min(lane, nrows));
+    rp1 = __ldg(p.rowptr + r0 + min(lane + 1, nrows));
+    return true;
+  }
+  __device__ __forceinline__ void advance() { ticket = __shfl_sync(0xffffffffu, next_ticket, 0); }
+  // planned kernels: the item's rows in the segment list, bit r of plan_mask[r / 32], clipped to nrows
+  __device__ __forceinline__ unsigned plan_defer_mask(const SpmmParams& p) const {
+    const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
+    return (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
+  }
+};
+
+// ---- a lane's columns in the row-per-warp kernels ---------------------------------------------------
+// Chunk ch of lane li starts at column k0 + (ch * LPR + li) * VEC; col_ok[ch]: it lies inside the row. row_bytes is
+// one dense row, lane_off the byte offset of the lane's first column in it, hcol (HEADS) the head of each chunk.
+template <typename X, int LPR, int VEC, int CH, bool HEADS>
+__device__ __forceinline__ void lane_cols(const SpmmParams& p, int li, bool (&col_ok)[CH], int (&hcol)[HEADS ? CH : 1],
+                                          uint32_t& row_bytes, int64_t& lane_off) {
+#pragma unroll
+  for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
+  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
+  row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
+  lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
+}
+
+// walk segment S (of batch b; B == 1 in the planned drain) with the row engine eng, which then holds the segment's
+// result in every lane group. The segment kernel and the planned drain both walk segments here, which is what makes
+// planned and unplanned products agree on the rows they defer. Each finishes a segment itself, in its own branch
+// order (the order decides their machine code): the row store for a whole row, else the fp32 partial.
+template <bool HEADS, typename Eng, typename T, int CH, int NH>
+__device__ __forceinline__ void walk_segment(Eng& eng, const SpmmParams& p, const Segment& S, int64_t b,
+                                             IndexRing<T>& ring, const bool (&col_ok)[CH], const int (&hcol)[NH],
+                                             uint32_t row_bytes, int64_t lane_off, int lane, int g, uint64_t pol) {
+  const int64_t base = S.start & ~(int64_t)31;
+  ring.reset(base, S.end);
+  const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
+  asm volatile("" : "+l"(matb));
+  eng.init();
+  set_scale(eng, p);
+  set_heads<HEADS>(eng, p, hcol);
+  eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
+  eng.reduce_groups();
+}
+
 // QO: e4m3 result with per-row scales (RowEngine::store_row_q8) instead of T. RES: plus an e4m3 residual per row.
 // HEADS: per-head weights (tsb200_spmm_heads); the ring then streams the column words only.
 template <typename T, int RED, int LPR, int CH, int U, int MINB, bool ACC = false, bool PLAN = false, typename X = T,
@@ -666,68 +754,36 @@ spmm_vec_kernel(const SpmmParams p) {
   const int g = lane / LPR, li = lane % LPR;
 
   IndexRing<T> ring;
-  ring.s_col = s_col[warp];
-  ring.s_val = s_val[warp];
-  ring.has_val = !HEADS && p.value != nullptr;
-  if (!HEADS && !ring.has_val) {  // has_value=false: the ring's value half is a constant 1
-    using VR = typename Vec<T>::vraw;
-    for (int i = lane; i < kRingAlloc; i += 32) reinterpret_cast<VR*>(s_val[warp])[i] = Vec<T>::one();
-    __syncwarp();
-  }
-  ring.col = p.col;
-  ring.val = HEADS ? nullptr : (const T*)p.value;
-  ring.limit = p.E;
+  ring.template bind<!HEADS>(p, s_col[warp], s_val[warp], lane);
   const uint64_t pol = make_policy_evict_last();
-
   bool col_ok[CH];
-#pragma unroll
-  for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
   int hcol[HEADS ? CH : 1];
-  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
-  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
+  uint32_t row_bytes;
+  int64_t lane_off;
+  lane_cols<X, LPR, VEC, CH, HEADS>(p, li, col_ok, hcol, row_bytes, lane_off);
 
-  const int item_rows = 1 << p.item_shift;
-  const int64_t nblk = (p.M + item_rows - 1) >> p.item_shift;
-  const int64_t n_items = nblk * p.B;
-
-  unsigned int item = 0;
-  if (lane == 0) item = atomicAdd(&p.counters[0], 1u);
-  item = __shfl_sync(0xffffffffu, item, 0);
-
-  while ((int64_t)item < n_items) {
-    unsigned int next_item = 0;
-    if (lane == 0) next_item = atomicAdd(&p.counters[0], 1u);  // latency hidden behind this item
-
-    const int64_t b = item / nblk, blk = item - b * nblk;
-    const int64_t r0 = blk << p.item_shift;
-    const int nrows = (int)min((int64_t)item_rows, p.M - r0);
-    const int64_t rp0 = __ldg(p.rowptr + r0 + min(lane, nrows));
-    const int64_t rp1 = __ldg(p.rowptr + r0 + min(lane + 1, nrows));
-    const int64_t a0 = __shfl_sync(0xffffffffu, rp0, 0);
+  for (WorkItem it(p, lane); it.start(p, lane); it.advance()) {
+    const int64_t a0 = __shfl_sync(0xffffffffu, it.rp0, 0);
     const int64_t base = a0 & ~(int64_t)31;
-    const int s_rel = (int)(rp0 - base), e_rel = (int)(rp1 - base);
+    const int s_rel = (int)(it.rp0 - base), e_rel = (int)(it.rp1 - base);
     const int deg = e_rel - s_rel;
 
     unsigned defer_mask;
     if constexpr (PLAN) {  // which rows are in the segment list was decided when the plan was built
-      const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
-      defer_mask = (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
+      defer_mask = it.plan_defer_mask(p);
     } else {
       const bool defer = defer_row(deg, lane);
       defer_mask = __ballot_sync(0xffffffffu, defer);
-      if (defer) push_row_segments(p, b, r0, lane, rp0, rp1, deg);  // rare
+      if (defer) push_row_segments(p, it.b, it.r0, lane, it.rp0, it.rp1, deg);  // rare
     }
     __syncwarp();
 
-    ring.reset(base, __shfl_sync(0xffffffffu, rp1, 31));  // lanes >= nrows hold the item's end
-    const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
+    ring.reset(base, __shfl_sync(0xffffffffu, it.rp1, 31));  // lanes >= nrows hold the item's end
+    const char* matb = (const char*)p.mat + it.b * p.N * (int64_t)row_bytes + lane_off;
     asm volatile("" : "+l"(matb));  // keep the gather base in a register
-    T* outb = (T*)p.out + (b * p.M + r0) * p.K + p.k0;
-    int64_t* argb = p.arg_out ? p.arg_out + (b * p.M + r0) * p.K + p.k0 : nullptr;
-    float* partb = ACC ? p.partial + (b * p.M + r0) * p.K + p.k0 : nullptr;
+    const RowOut<T, ACC, QO, RES> ro(p, it.b, it.r0);
 
-    for (int rl = 0; rl < nrows; rl++) {
+    for (int rl = 0; rl < it.nrows; rl++) {
       if ((defer_mask >> rl) & 1u) continue;
       const int s = __shfl_sync(0xffffffffu, s_rel, rl);
       const int e = __shfl_sync(0xffffffffu, e_rel, rl);
@@ -737,19 +793,8 @@ spmm_vec_kernel(const SpmmParams p) {
       set_heads<HEADS>(eng, p, hcol);
       eng.accumulate(ring, s, e, matb, row_bytes, col_ok, lane, g, pol);
       eng.reduce_groups();
-      if constexpr (QO) {
-        if (g == 0)
-          eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
-                                         argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li,
-                                         p.mean != 0, RES ? res_row(p, r0 + rl) : nullptr,
-                                         RES ? res_scale(p, r0 + rl) : 0.f);
-      } else {
-        if (g == 0) eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, e - s, p.E, col_ok, li, p.mean != 0,
-                                  ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0,
-                                  RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
-      }
+      if (g == 0) ro.store(eng, p, rl, e - s, col_ok, li);
     }
-    item = __shfl_sync(0xffffffffu, next_item, 0);
   }
 
   if constexpr (PLAN) {
@@ -758,22 +803,12 @@ spmm_vec_kernel(const SpmmParams p) {
     // combined by whichever warp finishes its last segment (counter per long row + fences, no waiting).
     constexpr int kcols = LPR * CH * VEC;
     while (true) {
-      unsigned int sidx = 0;
-      if (lane == 0) sidx = atomicAdd(&p.counters[5], 1u);
-      sidx = __shfl_sync(0xffffffffu, sidx, 0);
+      const unsigned int sidx = __shfl_sync(0xffffffffu, take_ticket(&p.counters[5], lane), 0);
       if ((int64_t)sidx >= p.n_seg) break;
       const Segment S = p.segs[sidx];
       const int64_t row = S.row_b;  // B == 1
-      const int64_t base = S.start & ~(int64_t)31;
-      ring.reset(base, S.end);
-      const char* matb = (const char*)p.mat + lane_off;
-      asm volatile("" : "+l"(matb));
       Eng eng;
-      eng.init();
-      set_scale(eng, p);
-      set_heads<HEADS>(eng, p, hcol);
-      eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
-      eng.reduce_groups();
+      walk_segment<HEADS>(eng, p, S, 0, ring, col_ok, hcol, row_bytes, lane_off, lane, g, pol);
       if (S.slot < 0) {
         if constexpr (QO) {
           if (g == 0)
@@ -838,53 +873,34 @@ spmm_gpr_kernel(const SpmmParams p) {
   head_cols<HEADS, LPR, VEC, 1>(hcol, p, li);
   const int hstride = HEADS ? p.heads : 1;  // value elements per entry
 
-  const int item_rows = 1 << p.item_shift;
-  const int64_t nblk = (p.M + item_rows - 1) >> p.item_shift;
-  const int64_t n_items = nblk * p.B;
-
-  unsigned int item = 0;
-  if (lane == 0) item = atomicAdd(&p.counters[0], 1u);
-  item = __shfl_sync(0xffffffffu, item, 0);
-
-  while ((int64_t)item < n_items) {
-    unsigned int next_item = 0;
-    if (lane == 0) next_item = atomicAdd(&p.counters[0], 1u);
-
-    const int64_t b = item / nblk, blk = item - b * nblk;
-    const int64_t r0 = blk << p.item_shift;
-    const int nrows = (int)min((int64_t)item_rows, p.M - r0);
-    const int64_t rp0 = __ldg(p.rowptr + r0 + min(lane, nrows));
-    const int64_t rp1 = __ldg(p.rowptr + r0 + min(lane + 1, nrows));
-    const int64_t base = __shfl_sync(0xffffffffu, rp0, 0);
-    const int s_rel = (int)(rp0 - base), e_rel = (int)(rp1 - base);
+  for (WorkItem it(p, lane); it.start(p, lane); it.advance()) {
+    const int64_t base = __shfl_sync(0xffffffffu, it.rp0, 0);
+    const int s_rel = (int)(it.rp0 - base), e_rel = (int)(it.rp1 - base);
     const int deg = e_rel - s_rel;
 
     unsigned defer_mask;
     if constexpr (PLAN) {
-      const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
-      defer_mask = (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
+      defer_mask = it.plan_defer_mask(p);
     } else {
       const bool defer = defer_row(deg, lane);
       defer_mask = __ballot_sync(0xffffffffu, defer);
-      if (defer) push_row_segments(p, b, r0, lane, rp0, rp1, deg);
+      if (defer) push_row_segments(p, it.b, it.r0, lane, it.rp0, it.rp1, deg);
     }
     __syncwarp();
 
-    const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
+    const char* matb = (const char*)p.mat + it.b * p.N * (int64_t)row_bytes + lane_off;
     asm volatile("" : "+l"(matb));
     const int64_t* __restrict__ colb = p.col + base;
     const T* __restrict__ valb = has_val ? (HEADS ? val + base * hstride + hcol[0] : val + base) : nullptr;
-    T* outb = (T*)p.out + (b * p.M + r0) * p.K + p.k0;
-    int64_t* argb = p.arg_out ? p.arg_out + (b * p.M + r0) * p.K + p.k0 : nullptr;
-    float* partb = ACC ? p.partial + (b * p.M + r0) * p.K + p.k0 : nullptr;
+    const RowOut<T, ACC, QO, RES> ro(p, it.b, it.r0);
     const bool col_ok_arr[1] = {col_ok};
     const int jbase = (int)base;  // absolute nnz index of ring-relative 0 (E < 2^31)
 
-    for (int t = 0; t < nrows; t += G) {
+    for (int t = 0; t < it.nrows; t += G) {
       const int rl = t + g;  // this lane group's row
       int s = __shfl_sync(0xffffffffu, s_rel, rl & 31);
       int e = __shfl_sync(0xffffffffu, e_rel, rl & 31);
-      const bool mine = rl < nrows && !((defer_mask >> (rl & 31)) & 1u);
+      const bool mine = rl < it.nrows && !((defer_mask >> (rl & 31)) & 1u);
       if (!mine) e = s;
       const int len = e - s;
       int maxlen = len;
@@ -943,19 +959,9 @@ spmm_gpr_kernel(const SpmmParams p) {
           else eng.minmax_step(eng.acc, eng.arg, V::vfloat(v[u]), d[u], jbase + s + j0 + u);
         }
       }
-      if constexpr (QO) {  // `mine` is the same for the LPR lanes of a group, so the group's amax shuffle is complete
-        if (mine)
-          eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
-                                         argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
-                                         p.mean != 0, RES ? res_row(p, r0 + rl) : nullptr,
-                                         RES ? res_scale(p, r0 + rl) : 0.f);
-      } else {
-        if (mine) eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, len, p.E, col_ok_arr, li,
-                                p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr, ACC ? p.acc_mode : 0,
-                                RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
-      }
+      // QO: `mine` is the same for the LPR lanes of a group, so the group's amax shuffle is complete
+      if (mine) ro.store(eng, p, rl, len, col_ok_arr, li);
     }
-    item = __shfl_sync(0xffffffffu, next_item, 0);
   }
 }
 
@@ -972,42 +978,21 @@ spmm_seg_kernel(const SpmmParams p) {
   const int g = lane / LPR, li = lane % LPR;
 
   IndexRing<T> ring;
-  ring.s_col = s_col[warp];
-  ring.s_val = s_val[warp];
-  ring.has_val = !HEADS && p.value != nullptr;
-  if (!HEADS && !ring.has_val) {  // has_value=false: the ring's value half is a constant 1
-    using VR = typename Vec<T>::vraw;
-    for (int i = lane; i < kRingAlloc; i += 32) reinterpret_cast<VR*>(s_val[warp])[i] = Vec<T>::one();
-    __syncwarp();
-  }
-  ring.col = p.col;
-  ring.val = HEADS ? nullptr : (const T*)p.value;
-  ring.limit = p.E;
+  ring.template bind<!HEADS>(p, s_col[warp], s_val[warp], lane);
   const uint64_t pol = make_policy_evict_last();
-
   bool col_ok[CH];
-#pragma unroll
-  for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
   int hcol[HEADS ? CH : 1];
-  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
-  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
-  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
+  uint32_t row_bytes;
+  int64_t lane_off;
+  lane_cols<X, LPR, VEC, CH, HEADS>(p, li, col_ok, hcol, row_bytes, lane_off);
 
   const int64_t nseg = p.plan_mask ? p.n_seg : min((int64_t)p.counters[1], p.seg_cap);
   const int64_t wstride = (int64_t)gridDim.x * kWarpsPerCta;
   for (int64_t sidx = (int64_t)blockIdx.x * kWarpsPerCta + warp; sidx < nseg; sidx += wstride) {
     const Segment S = p.segs[sidx];
     const int64_t b = S.row_b / p.M, row = S.row_b - b * p.M;
-    const int64_t base = S.start & ~(int64_t)31;
-    ring.reset(base, S.end);
-    const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
-    asm volatile("" : "+l"(matb));
     Eng eng;
-    eng.init();
-    set_scale(eng, p);
-    set_heads<HEADS>(eng, p, hcol);
-    eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
-    eng.reduce_groups();
+    walk_segment<HEADS>(eng, p, S, b, ring, col_ok, hcol, row_bytes, lane_off, lane, g, pol);
     if (g == 0) {
       if (S.slot < 0) {
         if constexpr (QO)
@@ -1017,10 +1002,10 @@ spmm_seg_kernel(const SpmmParams p) {
                                          RES ? res_scale(p, row) : 0.f);
         else
           eng.template store_row<RES>((T*)p.out + (b * p.M + row) * p.K + p.k0,
-                        p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
-                        S.end - S.start, p.E, col_ok, li, p.mean != 0,
-                        ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0,
-                        RES ? res_row(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
+                                      p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
+                                      S.end - S.start, p.E, col_ok, li, p.mean != 0,
+                                      ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0,
+                                      RES ? res_row(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
       } else {
         store_partial<LPR>(p, eng, S.slot, col_ok, li);
       }

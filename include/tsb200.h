@@ -355,6 +355,28 @@ TSB200_API int tsb200_segment_reduce_bw(const int64_t* seg, const int64_t* count
                                         int dtype, int reduce, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Segment softmax over a CSR / CSC pointer (torch.sparse.softmax over a row or a column; no counterpart in the
+ *   reference).  ptr i64[S+1] (rowptr, or colptr with perm = csr2csc); perm i64[E] or NULL; value, out dtype[E, D],
+ *   dtype F32 / F64 / F16 / BF16. Segment s is the entries j in [ptr[s], ptr[s+1]), read from value[perm ? perm[j] : j]
+ *   and written to out at the same position, so a column softmax comes back in CSR order. Per segment and column d,
+ *   in A = fp32 (fp64 for F64):
+ *     m = max_j v_j (any NaN gives NaN);  e_j = exp(fl(v_j - m));  S = sum_j e_j;  out_j = round(e_j / S) (IEEE
+ *     division). The order of the sum depends only on the segment's length and D, never on another segment, the grid
+ *     or the operands' alignment. A segment holding a NaN or +inf, or all -inf, gives NaN everywhere; a -inf entry
+ *     next to finite ones gives +0; an empty segment writes nothing.
+ *   tsb200_segment_softmax_bw: grad_in_j = round(out_j * (grad_out_j - sum_k out_k grad_out_k)), the dot in A by FMA
+ *     in a fixed order; out is the forward's result, grad_out / grad_in dtype[E, D] addressed like value / out.
+ *   No workspace, no atomics, no host synchronisation (graph-capturable). Returns TSB200_ERR_INVALID_ARG for a
+ *   negative extent or a NULL pointer that is needed, 0 without a launch when S, E or D is 0, and
+ *   TSB200_ERR_UNSUPPORTED for another dtype.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_segment_softmax(const int64_t* ptr, const int64_t* perm, const void* value, void* out, int64_t S,
+                                      int64_t E, int64_t D, int dtype, void* stream);
+TSB200_API int tsb200_segment_softmax_bw(const int64_t* ptr, const int64_t* perm, const void* out,
+                                         const void* grad_out, void* grad_in, int64_t S, int64_t E, int64_t D,
+                                         int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * COO coalesce.  Replaces torch_sparse.coalesce -> SparseStorage.__init__ sort + .coalesce()
  *   (torch_sparse/coalesce.py:5-25, torch_sparse/storage.py:149-162, 436-466).
  *   Phase 1 (tsb200_coalesce_sort): key = row*N + col, stable radix sort with the original position

@@ -74,6 +74,10 @@ SIGNATURES = {
                                       c_void_p]),
     "tsb200_segment_reduce_bw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
                                          c_int, c_int, c_void_p]),
+    "tsb200_segment_softmax": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int,
+                                       c_void_p]),
+    "tsb200_segment_softmax_bw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
+                                          c_int, c_void_p]),
     "tsb200_spspmm_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int64]),
     "tsb200_spspmm_symbolic": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
                                        c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),

@@ -641,6 +641,76 @@ def segment_reduce(ptr: Tensor, value: Tensor, reduce: str = "sum", perm: Option
     return _segment_reduce_raw(ptr, value, reduce, perm, want_arg=False)[0]
 
 
+def _segment_softmax_check(ptr: Tensor, value: Tensor, perm: Optional[Tensor]) -> None:
+    _check_cuda(ptr, "ptr")
+    _check_cuda(value, "value")
+    if perm is not None:
+        _check_cuda(perm, "perm")
+    if not value.dtype.is_floating_point or value.dtype not in _DTYPES:
+        raise RuntimeError(f'"softmax" not implemented for \'{value.dtype}\'')
+    if value.dim() == 0:
+        raise RuntimeError("softmax: value must be [E] or [E, *], got a 0-D tensor")
+    if perm is not None and perm.numel() != value.size(0):
+        raise RuntimeError(f"softmax: value must have {perm.numel()} rows (the nnz), got {value.size(0)}")
+
+
+def _segment_softmax_raw(ptr: Tensor, value: Tensor, perm: Optional[Tensor]) -> Tensor:
+    ptr, value = _i64(ptr, "ptr"), value.contiguous()
+    if perm is not None:
+        perm = _i64(perm, "perm")
+    out = torch.empty_like(value)
+    S, E = ptr.numel() - 1, value.size(0)
+    if S <= 0 or out.numel() == 0:
+        return out
+    with _on_device(value.device):
+        check(lib.tsb200_segment_softmax(_p(ptr), _p(perm), _p(value), _p(out), S, E, value.numel() // E,
+                                         _dtype_code(value.dtype), _stream(value.device)), "tsb200_segment_softmax")
+    return out
+
+
+def segment_softmax_bw(ptr: Tensor, out: Tensor, grad_out: Tensor, perm: Optional[Tensor]) -> Tensor:
+    """grad_in = out * (grad_out - sum over the segment of out * grad_out), per column (tsb200_segment_softmax_bw)."""
+    ptr, out, grad_out = _i64(ptr, "ptr"), out.contiguous(), grad_out.contiguous()
+    if perm is not None:
+        perm = _i64(perm, "perm")
+    grad_in = torch.empty_like(out)
+    S, E = ptr.numel() - 1, out.size(0)
+    if S <= 0 or out.numel() == 0:
+        return grad_in
+    with _on_device(out.device):
+        check(lib.tsb200_segment_softmax_bw(_p(ptr), _p(perm), _p(out), _p(grad_out), _p(grad_in), S, E,
+                                            out.numel() // E, _dtype_code(out.dtype), _stream(out.device)),
+              "tsb200_segment_softmax_bw")
+    return grad_in
+
+
+class _SegmentSoftmax(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, value, ptr, perm):
+        ptr = _i64(ptr, "ptr")
+        perm = None if perm is None else _i64(perm, "perm")
+        out = _segment_softmax_raw(ptr, value, perm)
+        ctx.save_for_backward(out, ptr, perm)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        out, ptr, perm = ctx.saved_tensors
+        return segment_softmax_bw(ptr, out, grad_out, perm), None, None
+
+
+def segment_softmax(ptr: Tensor, value: Tensor, perm: Optional[Tensor] = None) -> Tensor:
+    """Softmax of `value` [E] or [E, *] over each segment [ptr[s], ptr[s+1]), one per trailing column; with `perm`
+    (csr2csc, ptr = colptr) segment entry j is value[perm[j]], and the result is written back in `value`'s order.
+    bf16 / f16 / f32 / f64, fp32 arithmetic (fp64 for fp64); see tsb200_segment_softmax. Differentiable in `value`
+    once: the backward is one kernel over the saved result."""
+    _segment_softmax_check(ptr, value, perm)
+    if value.requires_grad and torch.is_grad_enabled():
+        return _SegmentSoftmax.apply(value, ptr, perm)
+    return _segment_softmax_raw(ptr, value, perm)
+
+
 class _PinnedScalar:
     """One pinned int64 per device-side count read back from the GPU (E', nnz(C)). The buffers are pooled:
     `read()` returns the value (after the caller synchronised the stream) and hands the buffer back."""

@@ -3,7 +3,7 @@
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
     torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant,
-                      quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads}  (own additions)
+                      quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads, segment_softmax}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -60,6 +60,8 @@ _EXTRA_SCHEMAS = {
                   "Tensor x, Tensor? row_csc) -> Tensor",
     "sddmm_heads": "(Tensor row, Tensor rowptr, Tensor col, Tensor? colptr, Tensor? csr2csc, Tensor? row_csc, "
                    "Tensor a, Tensor b) -> Tensor",
+    # softmax of value [E, *] over each segment of ptr (rowptr, or colptr with perm = csr2csc), per trailing column
+    "segment_softmax": "(Tensor ptr, Tensor value, Tensor? perm) -> Tensor",
 }
 
 
@@ -81,6 +83,7 @@ _EXTRA_IMPLS = {
     "quantize_fp8": ops.quantize_fp8,
     "sddmm": ops.sddmm, "sddmm_fp8": ops.sddmm_fp8,
     "spmm_heads": ops.spmm_heads, "sddmm_heads": ops.sddmm_heads,
+    "segment_softmax": ops.segment_softmax,
 }
 _IMPLS = {
     "spmm_sum": ops.spmm_sum, "spmm_mean": ops.spmm_mean, "spmm_min": ops.spmm_min, "spmm_max": ops.spmm_max,

@@ -410,20 +410,9 @@ sddmm_seg_kernel(const SpmmParams p, const X* __restrict__ grad, T* __restrict__
 template <typename T, int LPR, int CH, int U, int MINB, typename X = T, int HL = 0>
 static int launch_sddmm(SpmmParams p, const void* grad, void* out, cudaStream_t st, const float* gscale = nullptr,
                         uint32_t gstride = 0) {
-  auto* kmain = sddmm_vec_kernel<T, LPR, CH, U, MINB, X, HL>;
-  auto* kseg = sddmm_seg_kernel<T, LPR, CH, U, MINB, X, HL>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
-  const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
-  const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
-  p.item_shift = item_shift_for(p.M, grid_main);
-  const int64_t n_items = (p.M + (1 << p.item_shift) - 1) >> p.item_shift;
-  TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
-  const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);
-  kmain<<<gm, kWarpsPerCta * 32, 0, st>>>(p, (const X*)grad, (T*)out, gscale, gstride);
-  TSB_LAUNCH_CHECK();
-  kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p, (const X*)grad, (T*)out, gscale, gstride);
-  TSB_LAUNCH_CHECK();
-  return 0;
+  return launch_rowsplit(sddmm_vec_kernel<T, LPR, CH, U, MINB, X, HL>, sddmm_seg_kernel<T, LPR, CH, U, MINB, X, HL>,
+                         gc_main, gc_seg, p, st, (const X*)grad, (T*)out, gscale, gstride);
 }
 
 template <typename T> static int dispatch_sddmm(const SpmmParams& p, const void* grad, void* out, cudaStream_t st) {
@@ -619,41 +608,28 @@ extern "C" int tsb200_spmm_value_bw(const int64_t* row, const int64_t* rowptr, c
   if (B * K > 0 && (!mat || !grad)) return TSB200_ERR_INVALID_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const bool mean = reduce == TSB200_MEAN;
-  const size_t es = dtype_size(dtype);
+  const int64_t row_bytes = K * (int64_t)dtype_size(dtype);
+  // nnz-parallel vector kernel: 16-byte rows of mat and grad, gathered by 32-bit row and column indices
   const bool vec = (dtype == TSB200_F32 || dtype == TSB200_F16 || dtype == TSB200_BF16) && K > 0 &&
-                   (K * es) % 16 == 0 && !((uintptr_t)mat & 15) && !((uintptr_t)grad & 15) &&
-                   M < ((int64_t)1 << 32) && N < ((int64_t)1 << 32) && K * (int64_t)es < ((int64_t)1 << 31);
-  // row-wise path: single batch, >= 3 and <= 64 vectors per dense row, a workspace for the segment queue
-  const int64_t vecs = vec ? (K * (int64_t)es) / 16 : 0;
-  if (vec && B == 1 && vecs >= 3 && vecs <= 64 && E < ((int64_t)1 << 31) - 64 && !((uintptr_t)col & 7) && workspace &&
-      !((uintptr_t)workspace & 255)) {
-    const WsLayout L = ws_layout(1, K, E, false, false);
-    if (workspace_bytes >= L.total) {
-      SpmmParams p{rowptr, col, nullptr, mat, nullptr, nullptr, 1, M, N, K, E};
-      p.mean = mean ? 1 : 0;
-      bind_ws(p, (char*)workspace, L, false);
-      switch (dtype) {
-        case TSB200_F32: return dispatch_sddmm<float>(p, grad, out, st);
-        case TSB200_F16: return dispatch_sddmm<__half>(p, grad, out, st);
-        case TSB200_BF16: return dispatch_sddmm<__nv_bfloat16>(p, grad, out, st);
-      }
-    }
+                   row_bytes % 16 == 0 && rowsplit_aligned({mat, grad}, nullptr) && M < ((int64_t)1 << 32) &&
+                   N < ((int64_t)1 << 32) && row_bytes < ((int64_t)1 << 31);
+  // row-wise path: single batch, >= 3 and <= 64 vectors per dense row, a workspace for the segment queue; a short
+  // workspace falls back to the nnz-parallel kernel
+  if (vec && B == 1 && row_bytes >= 3 * 16 && row_bytes <= 64 * 16 && rowsplit_extents(E, N, row_bytes, M) &&
+      rowsplit_aligned({mat, grad}, col) && workspace && !((uintptr_t)workspace & 255)) {
+    SpmmParams p{rowptr, col, nullptr, mat, nullptr, nullptr, 1, M, N, K, E};
+    p.mean = mean ? 1 : 0;
+    if (!bind_unplanned(p, workspace, workspace_bytes, false, false))
+      return dispatch_vec_dtype(dtype, [&](auto tag) { return dispatch_sddmm<decltype(tag)>(p, grad, out, st); });
   }
-  if (vec) {
-    switch (dtype) {
-      case TSB200_F32: return dispatch_value_vec<float>(row, rowptr, col, mat, grad, out, B, M, N, K, E, mean, st);
-      case TSB200_F16: return dispatch_value_vec<__half>(row, rowptr, col, mat, grad, out, B, M, N, K, E, mean, st);
-      case TSB200_BF16:
-        return dispatch_value_vec<__nv_bfloat16>(row, rowptr, col, mat, grad, out, B, M, N, K, E, mean, st);
-    }
-  }
+  if (vec)
+    return dispatch_vec_dtype(dtype, [&](auto tag) {
+      return dispatch_value_vec<decltype(tag)>(row, rowptr, col, mat, grad, out, B, M, N, K, E, mean, st);
+    });
   return dispatch_dtype(dtype, [&](auto tag) -> int {
     using T = decltype(tag);
-    int64_t blocks = (E + 7) / 8;
-    const int64_t cap = (int64_t)num_sms() * 32;
-    if (blocks > cap) blocks = cap;
-    value_bw_generic_kernel<T><<<(int)blocks, 256, 0, st>>>(row, rowptr, col, (const T*)mat, (const T*)grad,
-                                                           (T*)out, B, M, N, K, E, mean);
+    value_bw_generic_kernel<T><<<warp_grid(E, 32), 256, 0, st>>>(row, rowptr, col, (const T*)mat, (const T*)grad,
+                                                                 (T*)out, B, M, N, K, E, mean);
     TSB_LAUNCH_CHECK();
     return 0;
   });
@@ -687,23 +663,15 @@ extern "C" int tsb200_sddmm_fp8(const int64_t* rowptr, const int64_t* col, const
     return 0;
   }
   if (!rowptr || !col || !a8 || !a_scale || !b8 || !b_scale) return TSB200_ERR_INVALID_ARG;
-  if (E >= ((int64_t)1 << 31) - 64 || N >= ((int64_t)1 << 32) || M >= ((int64_t)1 << 32)) return TSB200_ERR_UNSUPPORTED;
-  if (((uintptr_t)a8 & 15) || ((uintptr_t)b8 & 15) || ((uintptr_t)col & 7) || ((uintptr_t)a_scale & 3) ||
-      ((uintptr_t)b_scale & 3))
+  if (!rowsplit_extents(E, N, K, M) || !rowsplit_aligned({a8, b8}, col, {a_scale, b_scale}))
     return TSB200_ERR_UNSUPPORTED;
   if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
-  const WsLayout L = ws_layout(1, K, E, false, false);
-  if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
   SpmmParams p{rowptr, col, nullptr, b8, nullptr, nullptr, 1, M, N, K, E};
-  bind_ws(p, (char*)workspace, L, false);
+  if (const int rc = bind_unplanned(p, workspace, workspace_bytes, false, false)) return rc;
   p.scale = b_scale; p.scale_stride = (uint32_t)b_scale_stride;
-  const uint32_t as = (uint32_t)a_scale_stride;
-  switch (out_dtype) {
-    case TSB200_F32: return dispatch_sddmm_fp8<float>(p, a8, out, st, a_scale, as);
-    case TSB200_F16: return dispatch_sddmm_fp8<__half>(p, a8, out, st, a_scale, as);
-    case TSB200_BF16: return dispatch_sddmm_fp8<__nv_bfloat16>(p, a8, out, st, a_scale, as);
-  }
-  return TSB200_ERR_UNSUPPORTED;
+  return dispatch_vec_dtype(out_dtype, [&](auto tag) {
+    return dispatch_sddmm_fp8<decltype(tag)>(p, a8, out, st, a_scale, (uint32_t)a_scale_stride);
+  });
 }
 
 extern "C" int tsb200_spmm_minmax_bw(const int64_t* col, const void* value, const void* mat,
@@ -773,27 +741,19 @@ extern "C" int tsb200_sddmm_heads(const int64_t* rowptr, const int64_t* col, con
   const int64_t hl = (D * (int64_t)es) % 16 == 0 ? D * (int64_t)es / 16 : 0;
   const int64_t vecs = hl * H;
   const int64_t lpr = vecs <= 4 ? 4 : vecs <= 8 ? 8 : vecs <= 16 ? 16 : 32;
-  if (dtype != TSB200_F64 && hl > 0 && (hl & (hl - 1)) == 0 && hl <= lpr && vecs <= 64 &&
-      E < ((int64_t)1 << 31) - 64 && E * H < ((int64_t)1 << 40) && M < ((int64_t)1 << 32) &&
-      N < ((int64_t)1 << 32) && !((uintptr_t)a & 15) && !((uintptr_t)b & 15) && !((uintptr_t)col & 7) &&
-      !((uintptr_t)out % es) && workspace && !((uintptr_t)workspace & 255)) {
-    const WsLayout L = ws_layout(1, K, E, false, false);
-    if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+  if (dtype != TSB200_F64 && hl > 0 && (hl & (hl - 1)) == 0 && hl <= lpr && vecs <= 64 && E * H < ((int64_t)1 << 40) &&
+      rowsplit_extents(E, N, K * (int64_t)es, M) && rowsplit_aligned({a, b}, col) && !((uintptr_t)out % es) &&
+      workspace && !((uintptr_t)workspace & 255)) {
     SpmmParams p{rowptr, col, nullptr, b, nullptr, nullptr, 1, M, N, K, E};
     p.heads = (int)H;
-    bind_ws(p, (char*)workspace, L, false);
-    switch (dtype) {
-      case TSB200_F32: return dispatch_sddmm_heads<float>(p, (int)hl, a, out, st);
-      case TSB200_F16: return dispatch_sddmm_heads<__half>(p, (int)hl, a, out, st);
-      case TSB200_BF16: return dispatch_sddmm_heads<__nv_bfloat16>(p, (int)hl, a, out, st);
-    }
+    if (const int rc = bind_unplanned(p, workspace, workspace_bytes, false, false)) return rc;
+    return dispatch_vec_dtype(dtype,
+                              [&](auto tag) { return dispatch_sddmm_heads<decltype(tag)>(p, (int)hl, a, out, st); });
   }
   return dispatch_float_dtype(dtype, [&](auto tag) -> int {
     using T = decltype(tag);
-    int64_t blocks = (M + 7) / 8;
-    if (blocks > (int64_t)num_sms() * 32) blocks = (int64_t)num_sms() * 32;
-    sddmm_heads_generic_kernel<T><<<(int)blocks, 256, 0, st>>>(rowptr, col, (const T*)a, (const T*)b, (T*)out, M, H,
-                                                               D);
+    sddmm_heads_generic_kernel<T><<<warp_grid(M, 32), 256, 0, st>>>(rowptr, col, (const T*)a, (const T*)b, (T*)out,
+                                                                    M, H, D);
     TSB_LAUNCH_CHECK();
     return 0;
   });

@@ -1,9 +1,10 @@
 // spmm_common.cuh — pieces shared by the SpMM forward (spmm_fw.cu) and the row-wise SDDMM (spmm_bw.cu):
-// work-queue records, kernel parameters, the row-deferral rule, the per-warp cp.async index ring and the 16-byte
-// vector math.
+// work-queue records, kernel parameters, the row-deferral rule, the per-warp cp.async index ring, the 16-byte
+// vector math, and on the host the workspace binding, the row-split limits and launch, and the dtype switch.
 #pragma once
 
 #include <cstdlib>
+#include <initializer_list>
 
 #include "common.cuh"
 
@@ -393,6 +394,42 @@ static inline void bind_ws(SpmmParams& p, char* ws, const WsLayout& L, bool arg)
   p.part_arg = arg ? (int64_t*)(ws + L.part_arg) : nullptr;
   p.seg_cap = L.seg_cap; p.long_cap = L.long_cap; p.slot_cap = L.slot_cap;
 }
+// checks an unplanned workspace for p (layout ws_layout(p.B, p.K, p.E, ...)) and binds it: 0, TSB200_ERR_WORKSPACE
+// when it is missing or short, else TSB200_ERR_INVALID_ARG when it is not 256-byte aligned
+static inline int bind_unplanned(SpmmParams& p, void* workspace, size_t bytes, bool arg, bool partials = true) {
+  const WsLayout L = ws_layout(p.B, p.K, p.E, arg, partials);
+  if (!workspace || bytes < L.total) return TSB200_ERR_WORKSPACE;
+  if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
+  bind_ws(p, (char*)workspace, L, arg);
+  return 0;
+}
+
+// Extents the row-split kernels index in 32-bit arithmetic: E entries (an index ring reads up to 64 past the last), N
+// dense rows of row_bytes each, and M rows of a second dense operand where a kernel gathers those by row index.
+static inline bool rowsplit_extents(int64_t E, int64_t N, int64_t row_bytes, int64_t M = 0) {
+  return E < ((int64_t)1 << 31) - 64 && N < ((int64_t)1 << 32) && row_bytes < ((int64_t)1 << 31) &&
+         M < ((int64_t)1 << 32);
+}
+// Pointer alignments of the row-split kernels: dense operands, dense results and arg_out 16 B (vector loads and
+// stores), col 8 B (cp.async), values and scales 4 B. A NULL (absent) operand passes.
+static inline bool rowsplit_aligned(std::initializer_list<const void*> rows, const void* col,
+                                    std::initializer_list<const void*> words = {}) {
+  for (const void* r : rows)
+    if ((uintptr_t)r & 15) return false;
+  for (const void* w : words)
+    if ((uintptr_t)w & 3) return false;
+  return !((uintptr_t)col & 7);
+}
+
+// Runtime dtype -> compile-time type for the vector kernels (F32, F16, BF16); TSB200_ERR_UNSUPPORTED for any other.
+template <typename F> static inline int dispatch_vec_dtype(int dtype, F&& fn) {
+  switch (dtype) {
+    case TSB200_F32: return fn(float{});
+    case TSB200_F16: return fn(__half{});
+    case TSB200_BF16: return fn(__nv_bfloat16{});
+    default: return TSB200_ERR_UNSUPPORTED;
+  }
+}
 
 static inline int grid_for(const void* kernel, int threads) {
   int per_sm = 0;
@@ -430,6 +467,31 @@ static inline int item_shift_for(int64_t rows, int grid_main) {
   char* end = nullptr;
   const long v = strtol(ev, &end, 10);
   return (end != ev && *end == '\0' && v >= 0 && v <= 5) ? (int)v : s;
+}
+
+// The unplanned row-split launch: the work counters cleared, the main kernel over the row items, then the segment
+// kernel over the rows the main kernel deferred; `args` follow p in both kernels. The grid caches are the caller's,
+// one pair per kernel instantiation: a cache shared by two kernels would give one of them the other's grid.
+template <typename Kernel, typename... A>
+static int launch_rowsplit(Kernel* kmain, Kernel* kseg, GridCache& gc_main, GridCache& gc_seg, SpmmParams& p,
+                           cudaStream_t st, A... args) {
+  const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
+  const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
+  p.item_shift = item_shift_for(p.M * p.B, grid_main);
+  const int64_t n_items = ((p.M + (1 << p.item_shift) - 1) >> p.item_shift) * p.B;
+  TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
+  const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);
+  kmain<<<gm, kWarpsPerCta * 32, 0, st>>>(p, args...);
+  TSB_LAUNCH_CHECK();
+  kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p, args...);
+  TSB_LAUNCH_CHECK();
+  return 0;
+}
+
+// CTAs of 256 threads for a generic kernel that gives each of n_warps rows (or entries) a warp: one warp each, at most
+// cap_per_sm CTAs per SM
+static inline int warp_grid(int64_t n_warps, int cap_per_sm) {
+  return (int)min((n_warps + 7) / 8, (int64_t)num_sms() * cap_per_sm);
 }
 
 }  // namespace tsb

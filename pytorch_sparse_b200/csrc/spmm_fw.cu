@@ -1138,14 +1138,9 @@ spmm_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restric
 static bool vec_eligible(int dtype, int64_t K, int64_t E, int64_t N, const void* value,
                          const void* mat, const void* out, const void* col, const void* arg_out) {
   if (dtype != TSB200_F32 && dtype != TSB200_F16 && dtype != TSB200_BF16) return false;
-  const size_t es = dtype_size(dtype);
-  if ((K * es) % 16 != 0) return false;
-  if (E >= ((int64_t)1 << 31) - 64) return false;
-  if (N >= ((int64_t)1 << 32) || K * (int64_t)es >= ((int64_t)1 << 31)) return false;
-  if (((uintptr_t)mat & 15) || ((uintptr_t)out & 15) || ((uintptr_t)col & 7)) return false;
-  if (value && ((uintptr_t)value & 3)) return false;
-  if (arg_out && ((uintptr_t)arg_out & 15)) return false;
-  return true;
+  const int64_t row_bytes = K * (int64_t)dtype_size(dtype);
+  return row_bytes % 16 == 0 && rowsplit_extents(E, N, row_bytes) &&
+         rowsplit_aligned({mat, out, arg_out}, col, {value});
 }
 
 template <typename T, int RED, bool QO, bool RES = false>
@@ -1165,9 +1160,6 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
   constexpr int USEG = (U > LPR) ? LPR : U;  // the row engine needs U * (32 / LPR) <= 32
   auto* kseg = spmm_seg_kernel<T, RED, LPR, CH, USEG, MINB, ACC, X, QO, RES, HEADS>;
   static GridCache gc_main, gc_seg;  // per instantiation, per device
-  const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
-  p.item_shift = item_shift_for(p.M * p.B, grid_main);
-  const int64_t n_items = ((p.M + (1 << p.item_shift) - 1) >> p.item_shift) * p.B;
   for (int k0 = 0; k0 < p.K; k0 += kcols) {
     p.k0 = k0;
     if constexpr (PLAN) {
@@ -1175,6 +1167,9 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
       // then the plan's segments, drained by the same warps. The group-per-row kernel has no index ring to drain
       // with, so for narrow dense rows the segment / combine kernels are still launched — when the plan says there
       // is something for them to do.
+      const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
+      p.item_shift = item_shift_for(p.M * p.B, grid_main);
+      const int64_t n_items = ((p.M + (1 << p.item_shift) - 1) >> p.item_shift) * p.B;
       TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 256 + (size_t)p.n_long * 4, st));
       int64_t work = (n_items + kWarpsPerCta - 1) / kWarpsPerCta;
       if (!GPR) work = max(work, (p.n_seg + kWarpsPerCta - 1) / kWarpsPerCta);
@@ -1191,13 +1186,7 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
         }
       }
     } else {
-      const int grid_seg = gc_seg.get((const void*)kseg, kWarpsPerCta * 32);
-      TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 64, st));
-      const int gm = (int)min((int64_t)grid_main, (n_items + kWarpsPerCta - 1) / kWarpsPerCta);
-      kmain<<<gm, kWarpsPerCta * 32, 0, st>>>(p);
-      TSB_LAUNCH_CHECK();
-      kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
-      TSB_LAUNCH_CHECK();
+      if (const int rc = launch_rowsplit(kmain, kseg, gc_main, gc_seg, p, st)) return rc;
       launch_combine<T, RED, QO, RES>(p, kcols, st);
       TSB_LAUNCH_CHECK();
     }
@@ -1377,6 +1366,12 @@ static int bind_plan(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t
   p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
   return 0;
 }
+// a plan and its planned workspace, or else an unplanned workspace: 0 or the error code
+static int bind_workspace(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                          int64_t n_slot, void* workspace, size_t workspace_bytes, bool arg) {
+  return plan ? bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)
+              : bind_unplanned(p, workspace, workspace_bytes, arg);
+}
 
 // generic per-head SpMM (tsb200_spmm_heads off the vector path): warp per row, lane per column k of the H * D, the
 // entries summed in order with one rounding per product and per sum, as spmm_generic_kernel does
@@ -1410,12 +1405,8 @@ template <typename T, int RED>
 static int launch_generic(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
                           void* out, int64_t* arg_out, int64_t B, int64_t M, int64_t N, int64_t K,
                           int64_t E, bool mean, cudaStream_t st) {
-  const int64_t warps = B * M;
-  int64_t blocks = (warps + 7) / 8;
-  if (blocks > (int64_t)num_sms() * 64) blocks = (int64_t)num_sms() * 64;
-  if (blocks < 1) blocks = 1;
-  spmm_generic_kernel<T, RED><<<(int)blocks, 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)mat,
-                                                           (T*)out, arg_out, B, M, N, K, E, mean);
+  spmm_generic_kernel<T, RED><<<warp_grid(B * M, 64), 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)mat,
+                                                                    (T*)out, arg_out, B, M, N, K, E, mean);
   TSB_LAUNCH_CHECK();
   return 0;
 }
@@ -1446,16 +1437,9 @@ extern "C" int tsb200_spmm_fw(const int64_t* rowptr, const int64_t* col, const v
   cudaStream_t st = (cudaStream_t)stream;
 
   if (E > 0 && vec_eligible(dtype, K, E, N, value, mat, out, col, arg_out)) {
-    const WsLayout L = ws_layout(B, K, E, arg);
-    if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-    if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
     SpmmParams p{rowptr, col, value, mat, out, arg_out, B, M, N, K, E};
-    bind_ws(p, (char*)workspace, L, arg);
-    switch (dtype) {
-      case TSB200_F32: return dispatch_red_vec<float>(p, reduce, st);
-      case TSB200_F16: return dispatch_red_vec<__half>(p, reduce, st);
-      case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16>(p, reduce, st);
-    }
+    if (const int rc = bind_unplanned(p, workspace, workspace_bytes, arg)) return rc;
+    return dispatch_vec_dtype(dtype, [&](auto tag) { return dispatch_red_vec<decltype(tag)>(p, reduce, st); });
   }
 
   return dispatch_dtype(dtype, [&](auto tag) -> int {
@@ -1485,18 +1469,10 @@ extern "C" int tsb200_spmm_fw_acc(const int64_t* rowptr, const int64_t* col, con
   if (!vec_eligible(dtype, K, E, N, value, mat, acc_mode == 3 ? out : (void*)partial, col, nullptr))
     return TSB200_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
-  const WsLayout L = ws_layout(B, K, E, false);
-  if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-  if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
   SpmmParams p{rowptr, col, value, mat, out, nullptr, B, M, N, K, E};
   p.partial = partial; p.acc_mode = acc_mode;
-  bind_ws(p, (char*)workspace, L, false);
-  switch (dtype) {
-    case TSB200_F32: return dispatch_shape<float, R_SUM, true>(p, st);
-    case TSB200_F16: return dispatch_shape<__half, R_SUM, true>(p, st);
-    case TSB200_BF16: return dispatch_shape<__nv_bfloat16, R_SUM, true>(p, st);
-  }
-  return TSB200_ERR_UNSUPPORTED;
+  if (const int rc = bind_unplanned(p, workspace, workspace_bytes, false)) return rc;
+  return dispatch_vec_dtype(dtype, [&](auto tag) { return dispatch_shape<decltype(tag), R_SUM, true>(p, st); });
 }
 
 // ---- planned SpMM: the segment structure of a matrix is computed once and reused by every product --------------
@@ -1515,12 +1491,9 @@ extern "C" int tsb200_spmm_plan(const int64_t* rowptr, int64_t M, int64_t E, voi
   char* pl = (char*)plan;
   TSB_CUDA_TRY(cudaMemsetAsync(pl + L.header, 0, 256, st));
   if (M > 0) {
-    int64_t blocks = (((M + 31) / 32) * 32 + 255) / 256;
-    const int64_t cap = (int64_t)num_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    spmm_plan_kernel<<<(int)blocks, 256, 0, st>>>(rowptr, M, (uint32_t*)(pl + L.mask), (Segment*)(pl + L.segs),
-                                                 (uint32_t*)(pl + L.seg_lr), (LongRow*)(pl + L.longs),
-                                                 (unsigned int*)(pl + L.header), L.seg_cap, L.long_cap);
+    spmm_plan_kernel<<<warp_grid((M + 31) / 32, 16), 256, 0, st>>>(
+        rowptr, M, (uint32_t*)(pl + L.mask), (Segment*)(pl + L.segs), (uint32_t*)(pl + L.seg_lr),
+        (LongRow*)(pl + L.longs), (unsigned int*)(pl + L.header), L.seg_cap, L.long_cap);
     TSB_LAUNCH_CHECK();
   }
   if (counts_host) {  // [n_seg, n_long, n_slot] as uint32 counters 1..3 of the header; the caller widens them
@@ -1551,14 +1524,10 @@ extern "C" int tsb200_spmm_fw_planned(const int64_t* rowptr, const int64_t* col,
   if (!rowptr || !col || !mat || !out || !plan || (arg && !arg_out)) return TSB200_ERR_INVALID_ARG;
   if (!vec_eligible(dtype, K, E, N, value, mat, out, col, arg_out)) return TSB200_ERR_UNSUPPORTED;
   SpmmParams p{rowptr, col, value, mat, out, arg_out, 1, M, N, K, E};
-  if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)) return rc;
+  if (const int rc = bind_workspace(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg))
+    return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case TSB200_F32: return dispatch_red_vec<float, true>(p, reduce, st);
-    case TSB200_F16: return dispatch_red_vec<__half, true>(p, reduce, st);
-    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, true>(p, reduce, st);
-  }
-  return TSB200_ERR_UNSUPPORTED;
+  return dispatch_vec_dtype(dtype, [&](auto tag) { return dispatch_red_vec<decltype(tag), true>(p, reduce, st); });
 }
 
 // ---- SpMM over an fp8 (e4m3) dense operand with per-tensor or per-row scales ----------------------------------------
@@ -1597,12 +1566,9 @@ __global__ void __launch_bounds__(256) spmm_res_only_kernel(const SpmmParams p) 
 template <bool PLAN, bool QO, bool RES = false>
 static int dispatch_fp8_out(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
   if constexpr (QO) return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, true, RES>(p, reduce, st);
-  switch (out_dtype) {
-    case TSB200_F32: return dispatch_red_vec<float, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
-    case TSB200_F16: return dispatch_red_vec<__half, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
-    case TSB200_BF16: return dispatch_red_vec<__nv_bfloat16, PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
-  }
-  return TSB200_ERR_UNSUPPORTED;
+  return dispatch_vec_dtype(out_dtype, [&](auto tag) {
+    return dispatch_red_vec<decltype(tag), PLAN, __nv_fp8_e4m3, false, RES>(p, reduce, st);
+  });
 }
 template <bool PLAN, bool QO>
 static int dispatch_fp8_res(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
@@ -1623,8 +1589,8 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
                             const float* scale, int64_t scale_stride, void* out, float* out_scale, int64_t* arg_out,
                             int64_t M, int64_t N, int64_t K, int64_t E, int out_dtype, int reduce, const void* plan,
                             size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
-                            size_t workspace_bytes, void* stream, const uint8_t* res8 = nullptr,
-                            const float* res_scale = nullptr, int64_t res_stride = 0) {
+                            size_t workspace_bytes, void* stream, const uint8_t* res8, const float* res_scale,
+                            int64_t res_stride) {
   if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
   if (reduce < TSB200_SUM || reduce > TSB200_MAX) return TSB200_ERR_INVALID_ARG;
   if (scale_stride != 0 && scale_stride != 1) return TSB200_ERR_INVALID_ARG;
@@ -1648,12 +1614,7 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
     if (E == 0 && K > 0) {  // every row is empty: the result is the residual alone
       if ((uintptr_t)out & 15) return TSB200_ERR_UNSUPPORTED;
       if constexpr (QO) return launch_res_only<float, true>(p, st);
-      switch (out_dtype) {
-        case TSB200_F32: return launch_res_only<float, false>(p, st);
-        case TSB200_F16: return launch_res_only<__half, false>(p, st);
-        case TSB200_BF16: return launch_res_only<__nv_bfloat16, false>(p, st);
-      }
-      return TSB200_ERR_UNSUPPORTED;
+      return dispatch_vec_dtype(out_dtype, [&](auto tag) { return launch_res_only<decltype(tag), false>(p, st); });
     }
   }
   if (E == 0 || K == 0) {  // every row is empty: 0, arg_out = E = 0, and a scale of 1 (an amax of 0)
@@ -1668,20 +1629,14 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
     return 0;
   }
   if (!col || !mat || !scale) return TSB200_ERR_INVALID_ARG;
-  if (E >= ((int64_t)1 << 31) - 64 || N >= ((int64_t)1 << 32) || K >= ((int64_t)1 << 31)) return TSB200_ERR_UNSUPPORTED;
-  if (((uintptr_t)mat & 15) || ((uintptr_t)out & 15) || ((uintptr_t)col & 7) || ((uintptr_t)scale & 3))
+  if (!rowsplit_extents(E, N, K) || !rowsplit_aligned({mat, out, arg_out}, col, {value, scale}))
     return TSB200_ERR_UNSUPPORTED;
-  if ((value && ((uintptr_t)value & 3)) || (arg_out && ((uintptr_t)arg_out & 15))) return TSB200_ERR_UNSUPPORTED;
   if (!workspace || ((uintptr_t)workspace & 255)) return TSB200_ERR_INVALID_ARG;
-  if (plan) {  // planned: the layout of tsb200_spmm_fw_planned
-    if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)) return rc;
-    return dispatch_fp8_res<true, QO>(p, out_dtype, reduce, st);
-  }
-  // unplanned: the layout of tsb200_spmm_fw (tsb200_spmm_fw_workspace_bytes(1, M, K, E, out_dtype, reduce))
-  const WsLayout L = ws_layout(1, K, E, arg);
-  if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-  bind_ws(p, (char*)workspace, L, arg);
-  return dispatch_fp8_res<false, QO>(p, out_dtype, reduce, st);
+  // the workspace layouts of tsb200_spmm_fw_planned and, without a plan, tsb200_spmm_fw
+  if (const int rc = bind_workspace(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg))
+    return rc;
+  return plan ? dispatch_fp8_res<true, QO>(p, out_dtype, reduce, st)
+              : dispatch_fp8_res<false, QO>(p, out_dtype, reduce, st);
 }
 }  // namespace tsb
 
@@ -1692,7 +1647,7 @@ extern "C" int tsb200_spmm_fw_fp8(const int64_t* rowptr, const int64_t* col, con
                                   size_t workspace_bytes, void* stream) {
   return spmm_fw_fp8_impl<false>(rowptr, col, value, mat, scale, scale_stride, out, nullptr, arg_out, M, N, K, E,
                                  out_dtype, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes,
-                                 stream);
+                                 stream, nullptr, nullptr, 0);
 }
 
 extern "C" int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
@@ -1702,7 +1657,7 @@ extern "C" int tsb200_spmm_fw_fp8_quant(const int64_t* rowptr, const int64_t* co
                                         int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream) {
   return spmm_fw_fp8_impl<true>(rowptr, col, value, mat, scale, scale_stride, out8, out_scale, arg_out, M, N, K, E,
                                 TSB200_F32, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace,
-                                workspace_bytes, stream);
+                                workspace_bytes, stream, nullptr, nullptr, 0);
 }
 
 extern "C" int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
@@ -1753,28 +1708,17 @@ extern "C" int tsb200_spmm_heads(const int64_t* rowptr, const int64_t* col, cons
       H * E < ((int64_t)1 << 31)) {
     SpmmParams p{rowptr, col, value, x, out, nullptr, 1, M, N, K, E};
     p.heads = (int)H;
-    if (plan) {
-      if (const int rc = bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, false))
-        return rc;
-    } else {
-      const WsLayout L = ws_layout(1, K, E, false);
-      if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
-      if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
-      bind_ws(p, (char*)workspace, L, false);
-    }
-    switch (dtype) {
-      case TSB200_F32: return plan ? dispatch_heads<float, true>(p, st) : dispatch_heads<float, false>(p, st);
-      case TSB200_F16: return plan ? dispatch_heads<__half, true>(p, st) : dispatch_heads<__half, false>(p, st);
-      case TSB200_BF16:
-        return plan ? dispatch_heads<__nv_bfloat16, true>(p, st) : dispatch_heads<__nv_bfloat16, false>(p, st);
-    }
+    if (const int rc = bind_workspace(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, false))
+      return rc;
+    return dispatch_vec_dtype(dtype, [&](auto tag) {
+      using T = decltype(tag);
+      return plan ? dispatch_heads<T, true>(p, st) : dispatch_heads<T, false>(p, st);
+    });
   }
   return dispatch_float_dtype(dtype, [&](auto tag) -> int {
     using T = decltype(tag);
-    int64_t blocks = (M + 7) / 8;
-    if (blocks > (int64_t)num_sms() * 64) blocks = (int64_t)num_sms() * 64;
-    spmm_heads_generic_kernel<T><<<(int)blocks, 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)x, (T*)out, M,
-                                                              H, D);
+    spmm_heads_generic_kernel<T><<<warp_grid(M, 64), 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)x,
+                                                                   (T*)out, M, H, D);
     TSB_LAUNCH_CHECK();
     return 0;
   });

@@ -30,8 +30,6 @@
 //     value tells the product whether it was the first on its column (the symbolic pass just counts those),
 //     values with L2 atomics straight into val_c.
 // Everything is HBM-bound on the 16+s bytes per output nonzero that must be written.
-#include <cstdlib>
-
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -44,14 +42,14 @@ constexpr int kFlatU = 8;                         // products per thread on the 
 constexpr int kStageCap = kFlatU * kSpThreads;    // output entries staged in shared memory per row (2048)
 constexpr int kMaxWindowLog2 = 18;
 constexpr int kMaxWindowBits = 1 << kMaxWindowLog2;
-constexpr int kClaimSlotDefault = 3;              // single-pass mode: schedule slot of the next row's ticket (see the kernel)
+constexpr int kClaimSlot = 3;                     // single-pass mode: schedule slot of the next row's ticket (SpNext)
 constexpr int kABatch = 128;                      // A entries staged per batch
 static_assert(kStageCap <= (1 << (32 - kMaxWindowLog2 - 1)), "owner id and column share one 32-bit word");
 
 struct SpParams {
   const int64_t* rowptr_a; const int64_t* col_a; const void* val_a;
   const int64_t* rowptr_b; const int64_t* col_b; const void* val_b;
-  int64_t M, Kd, N;
+  int64_t M, N;
   int64_t* counts;          // symbolic: per-row nnz (accumulated at rowptr_c + 1, pre-zeroed)
   const int64_t* rowptr_c;  // numeric
   int64_t* row_c; int64_t* col_c; void* val_c;
@@ -59,8 +57,9 @@ struct SpParams {
   unsigned long long* status;  // FUSED: per-row look-back words (zeroed by the host)
   int64_t capacity;            // FUSED: entries the output arrays can hold
   int* overflow;               // FUSED: set when a row would not fit
-  unsigned long long* dbg;     // FUSED: optional look-back statistics (steps, empty polls, look-backs)
-  int claim_slot;              // where in a row's schedule the NEXT row's ticket is taken (0 = at the start)
+  // FUSED: kClaimSlot, read at run time: compiled in as a constant it made the C4 single pass take 8.4-8.7 ms instead
+  // of 7.1-7.2 ms (one H100 80GB HBM3 at a 700 W power limit), although ptxas then reports no spills
+  int claim_slot;
   int window_bits;  // power of two, 1024 .. 2^18
   int log2_wpt;     // log2(bitmap words per scan chunk), 2..5; chunks = (window_bits/32) >> log2_wpt <= 256
 };
@@ -212,18 +211,14 @@ __device__ __forceinline__ void sp_st_status(unsigned long long* q, unsigned lon
 // One warp: number of output entries of all rows < i. Lane l inspects row j - l; a row that has published its
 // inclusive prefix ends the walk. Rows are claimed in increasing order by CTAs that are running, and a row's
 // aggregate depends on no other row, so every predecessor's status eventually becomes non-zero.
-__device__ __forceinline__ int64_t sp_lookback(const unsigned long long* status, int64_t i, int lane,
-                                               unsigned long long* dbg) {
+__device__ __forceinline__ int64_t sp_lookback(const unsigned long long* status, int64_t i, int lane) {
   int64_t excl = 0;
-  unsigned steps = 0, polls = 0;
   for (int64_t j = i - 1; j >= 0; j -= 32) {
     const int64_t r = j - lane;
     unsigned long long st = kStPrefix;  // rows before row 0: inclusive prefix 0
-    steps++;
     if (r >= 0) {
       st = sp_ld_status(status + r);
       while ((st >> 62) == 0) {
-        polls++;
         __nanosleep(40);
         st = sp_ld_status(status + r);
       }
@@ -236,16 +231,172 @@ __device__ __forceinline__ int64_t sp_lookback(const unsigned long long* status,
     excl += v;
     if (pm) break;
   }
-  if (dbg) {  // tuning aid (TSB200_SPSPMM_DEBUG): look-back steps and status polls that found nothing yet
+  return excl;
+}
+
+// Single pass, warp 0 of a row with n > 0 output entries: finds the row's start by look-back, publishes its inclusive
+// prefix and leaves the start in s_base, or -1 when the row does not fit into `capacity` (then the overflow flag is set
+// and nothing of the row may be written; cannot happen with capacity >= the number of products).
+__device__ __forceinline__ void sp_place(const SpParams& p, int64_t i, int64_t n, int lane, long long& s_base) {
+  const int64_t base = sp_lookback(p.status, i, lane);
+  if (lane == 0) {
+    sp_st_status(p.status + i, kStPrefix | (unsigned long long)(base + n));
+    const bool fits = base + n <= p.capacity;
+    if (!fits) *p.overflow = 1;
+    s_base = fits ? base : -1;
+  }
+}
+
+__device__ __forceinline__ int sp_warp_sum(int v) {
 #pragma unroll
-    for (int off = 16; off; off >>= 1) polls += __shfl_xor_sync(0xffffffffu, polls, off);
-    if (lane == 0) {
-      atomicAdd(dbg, (unsigned long long)steps);
-      atomicAdd(dbg + 1, (unsigned long long)polls);
-      atomicAdd(dbg + 2, 1ull);
+  for (int off = 16; off; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+
+// symbolic: add the columns this warp's threads were first on to counts[i]
+__device__ __forceinline__ void sp_store_count(const SpParams& p, int64_t i, int cnt) {
+  cnt = sp_warp_sum(cnt);
+  if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(reinterpret_cast<unsigned long long*>(p.counts + i), (unsigned long long)cnt);
+}
+
+// The next row's A-row metadata, prefetched while the current row runs: B-row start, length and a_ik of A entry tid
+template <typename T>
+struct SpPrefetch {
+  bool valid;
+  int64_t bs;
+  int len;
+  T av;
+};
+
+// The next row, one row ahead: ticket taken at slot slot0 of the current row, read after the next barrier, then its loads
+// rowptr_a -> col_a -> rowptr_b / val_a at the two slots after. Slot 0 = row start; in single-pass mode a later slot
+// shortens the time from ticket to published nnz, which the rows behind the next row wait for.
+template <bool NUMERIC, typename T>
+struct SpNext {
+  const SpParams& p;
+  int slot0;              // the slot at which the next row's ticket is taken
+  unsigned int* s_claim;  // row tickets: s_claim[par] the row being processed, s_claim[par ^ 1] the next one
+  int par;
+  SpPrefetch<T>& pf;
+  int64_t row, s = 0, e = 0;  // the next row and its A-row extent
+  bool do_pf = false;     // the next row is one A batch: its metadata is prefetched
+  int64_t k = -1;         // column of the next row's A entry tid (-1: none)
+  int stage = 0;          // 0 nothing yet, 1 ticket taken, 2 row known, 3 its col_a issued, 4 its rowptr_b issued
+
+  __device__ __forceinline__ SpNext(const SpParams& p, int slot0, unsigned int* s_claim, int par, SpPrefetch<T>& pf)
+      : p(p), slot0(slot0), s_claim(s_claim), par(par), pf(pf), row(p.M) {}
+  __device__ __forceinline__ void take() {
+    if (threadIdx.x == 0) s_claim[par ^ 1] = atomicAdd(p.counter, 1u);
+    stage = 1;
+  }
+  __device__ __forceinline__ void read() {
+    row = s_claim[par ^ 1];
+    if (row < p.M) { s = p.rowptr_a[row]; e = p.rowptr_a[row + 1]; }
+    stage = 2;
+  }
+  // the step due at slot `slot` of the current row
+  __device__ __forceinline__ void at(int slot) {
+    const int tid = threadIdx.x;
+    if (stage == 0 && slot0 <= slot) {
+      take();
+    } else if (stage == 1) {
+      read();
+    } else if (stage == 2) {
+      const int64_t nn = e - s;
+      if (nn > 0 && nn <= kABatch) {
+        do_pf = true;
+        if (tid < nn) k = p.col_a[s + tid];
+      }
+      stage = 3;
+    } else if (stage == 3) {
+      if (do_pf) {
+        if (k >= 0) {
+          const T* va = reinterpret_cast<const T*>(p.val_a);
+          pf.bs = p.rowptr_b[k];
+          pf.len = (int)(p.rowptr_b[k + 1] - pf.bs);
+          pf.av = (NUMERIC && va) ? va[s + tid] : (T)1;
+        }
+        pf.valid = true;
+      }
+      stage = 4;
     }
   }
-  return excl;
+  // what the current row's path did not reach: ticket and row extent are needed, the prefetch is not (see staging)
+  __device__ __forceinline__ void finish() {
+    if (stage == 0) take();
+    if (stage == 1) {
+      __syncthreads();
+      read();
+    }
+  }
+};
+
+// The products of A row [a_s, a_e) on the general path. Its A entries are staged kABatch at a time in s_bs / s_len /
+// s_av (a row of one batch was staged at its start); one warp per A entry, lanes striding its B row.
+template <bool NUMERIC, typename T>
+struct SpWalk {
+  const SpParams& p;
+  int64_t a_s, a_e;
+  bool single_batch;
+  int64_t* s_bs;
+  int* s_len;
+  T* s_av;
+  uint64_t pol_b;
+
+  // body(c, c0 = c - wlo, A entry in the staged batch, index into B) for every product with column c in [wlo, whi)
+  template <typename Body>
+  __device__ __forceinline__ void operator()(int64_t wlo, int64_t whi, Body&& body) const {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const T* va = reinterpret_cast<const T*>(p.val_a);
+    for (int64_t ab = a_s; ab < a_e; ab += kABatch) {
+      const int na = (int)min((int64_t)kABatch, a_e - ab);
+      if (!single_batch) {
+        __syncthreads();
+        if (tid < na) {
+          const int64_t k = p.col_a[ab + tid];
+          const int64_t kb = p.rowptr_b[k];
+          s_bs[tid] = kb;
+          s_len[tid] = (int)(p.rowptr_b[k + 1] - kb);
+          if (NUMERIC) s_av[tid] = va ? va[ab + tid] : (T)1;
+        }
+        __syncthreads();
+      }
+      for (int e = warp; e < na; e += kSpWarps) {
+        const int64_t ebs = s_bs[e];
+        const int elen = s_len[e];
+        for (int f = lane; f < elen; f += 32) {
+          const int64_t c = (int64_t)ldg64_hint(p.col_b + ebs + f, pol_b);
+          if (c >= wlo && c < whi) body(c, (uint32_t)(c - wlo), e, ebs + f);
+        }
+      }
+    }
+  }
+};
+
+// Counting pass over the windows [win_lo, win_hi] (the whole job of the symbolic kernel; in single-pass mode it gives
+// the row's nnz before anything is written): every product marks its column with atomicOr, whose return value tells it
+// whether it was first. Returns the number of columns this thread was first on; the touched chunks are cleared again.
+template <bool NUMERIC, typename T>
+__device__ __forceinline__ int sp_count_pass(const SpWalk<NUMERIC, T>& walk, int64_t win_lo, int64_t win_hi,
+                                             int64_t W, uint32_t* bitmap, unsigned char* tflag, int lw, uint32_t nch) {
+  const int tid = threadIdx.x;
+  int cnt = 0;
+  for (int64_t win = win_lo; win <= win_hi; win++) {
+    const int64_t wlo = win * W;
+    walk(wlo, wlo + W, [&](int64_t, uint32_t c0, int, int64_t) {
+      const uint32_t bit = 1u << (c0 & 31u);
+      const uint32_t old = atomicOr(&bitmap[sp_phys(c0 >> 5)], bit);
+      if (!(old & bit)) cnt++;
+      tflag[c0 >> (5 + lw)] = 1;
+    });
+    __syncthreads();
+    if ((uint32_t)tid < nch && tflag[tid]) {
+      sp_count_clear_chunk(bitmap, lw);
+      tflag[tid] = 0;
+    }
+    __syncthreads();
+  }
+  return cnt;
 }
 
 template <int MODE, typename T>
@@ -286,77 +437,31 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
   // B is re-read nnz(A)/Kd times while 20 bytes per output nonzero stream through L2: keep B's lines (evict_last)
   const uint64_t pol_b = make_policy_evict_last();
 
-  // next row's A-row metadata, prefetched into registers while the current row is processed
-  bool pf_valid = false;
-  int64_t pf_bs = 0;
-  int pf_len = 0;
-  T pf_av = (T)1;
+  SpPrefetch<T> pf{false, 0, 0, (T)1};
 
   __syncthreads();
-  // Rows are handed out one at a time from a global ticket counter, one row AHEAD: the ticket of the next row is
-  // taken when a row starts, so its rowptr_a -> col_a -> rowptr_b chain of dependent loads overlaps this row's work.
   int par = 0;
   int64_t i = s_claim[0];
   int64_t a_s = 0, a_e = 0;
   if (i < p.M) { a_s = p.rowptr_a[i]; a_e = p.rowptr_a[i + 1]; }
 
-  // The next row's ticket is taken at schedule slot `cs` of the current row, read after the following barrier
-  // (slot cs + 1), and its metadata chain is issued at slots cs + 2 / cs + 3. Slot 0 = row start (longest prefetch
-  // distance); later slots shorten the time between taking a ticket and publishing that row's nnz, which is what
-  // the rows behind it wait for in single-pass mode.
-  const int cs = FUSED ? p.claim_slot : 0;
   while (i < p.M) {
     const int64_t n_a = a_e - a_s;
-    int64_t nrow = p.M, nx_s = 0, nx_e = 0;   // the next row and its A-row extent
-    bool do_pf = false;
-    int64_t nk = -1;
-    int stage = 0;  // 0 nothing yet, 1 ticket taken, 2 next row known, 3 its col_a issued, 4 its rowptr_b issued
-
-#define SP_NEXT_ROW()                                              \
-  nrow = s_claim[par ^ 1];                                         \
-  if (nrow < p.M) { nx_s = p.rowptr_a[nrow]; nx_e = p.rowptr_a[nrow + 1]; }
-#define SP_PF_STAGE1()                                             \
-  {                                                                \
-    const int64_t nn = nx_e - nx_s;                                \
-    if (nn > 0 && nn <= kABatch) {                                 \
-      do_pf = true;                                                \
-      if (tid < nn) nk = p.col_a[nx_s + tid];                      \
-    }                                                              \
-  }
-#define SP_PF_STAGE2()                                             \
-  if (do_pf) {                                                     \
-    if (nk >= 0) {                                                 \
-      pf_bs = p.rowptr_b[nk];                                      \
-      pf_len = (int)(p.rowptr_b[nk + 1] - pf_bs);                  \
-      pf_av = (NUMERIC && va) ? va[nx_s + tid] : (T)1;             \
-    }                                                              \
-    pf_valid = true;                                               \
-  }
-
-#define SP_AT(S)                                                                             \
-  {                                                                                          \
-    if (stage == 0 && cs <= (S)) {                                                           \
-      if (tid == 0) s_claim[par ^ 1] = atomicAdd(p.counter, 1u);                             \
-      stage = 1;                                                                             \
-    } else if (stage == 1) { SP_NEXT_ROW(); stage = 2; }                                     \
-    else if (stage == 2) { SP_PF_STAGE1(); stage = 3; }                                      \
-    else if (stage == 3) { SP_PF_STAGE2(); stage = 4; }                                      \
-  }
-
+    SpNext<NUMERIC, T> nx(p, FUSED ? p.claim_slot : 0, s_claim, par, pf);
     do {  // one row; `break` = done with it
       if (n_a <= 0) {  // empty row: counts[i] stays 0 (pre-zeroed) / status = aggregate 0; no output
         if (FUSED && tid == 0) sp_st_status(p.status + i, kStAgg);
-        pf_valid = false;
+        pf.valid = false;
         break;
       }
-      SP_AT(0);
+      nx.at(0);
       const int na0 = (int)min(n_a, (int64_t)kABatch);
 
       // ---- stage the (first batch of the) A-row metadata: start/length of each B row, a_ik; number the products ----
       int64_t bs = 0;
       int len = 0;
       T av = (T)1;
-      if (pf_valid) { bs = pf_bs; len = pf_len; av = pf_av; }
+      if (pf.valid) { bs = pf.bs; len = pf.len; av = pf.av; }
       else if (tid < na0) {
         const int64_t k = p.col_a[a_s + tid];
         bs = p.rowptr_b[k];
@@ -372,14 +477,14 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
       const int len_c = min(len, kStageCap + 1);  // keeps the sum in range; any clamped length disables the flat path
       int P;
       const int excl = sp_block_scan(len_c, s_warp, P);
-      SP_AT(1);   // (slot 0 ticket: the barrier inside the scan made it visible; the two rowptr_a loads are in flight)
+      nx.at(1);  // (slot 0 ticket: the barrier inside the scan made it visible; the two rowptr_a loads are in flight)
       if (tid < na0) {
         s_se[tid] = make_int2(excl, excl + len_c);
         // the 32-aligned product numbers inside [excl, excl + len): this entry is where their chunk starts
         if (P <= kStageCap)
           for (int k = (excl + 31) >> 5; (k << 5) < excl + len_c; k++) s_ent[k] = (unsigned char)tid;
       }
-      pf_valid = false;
+      pf.valid = false;
       __syncthreads();  // s_bs / s_len / s_se / s_ent / s_av visible
 
       const bool flat = !multi_window && n_a <= kABatch && P <= kStageCap;
@@ -404,22 +509,19 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
             }
           }
         }
-        SP_AT(2);
+        nx.at(2);
 #pragma unroll
         for (int u = 0; u < kFlatU; u++)
           if (cc[u] != 0xffffffffu) sp_mark(bitmap, cc[u]);
         __syncthreads();
-        SP_AT(3);
+        nx.at(3);
 #pragma unroll
         for (int u = 0; u < kFlatU; u++)
           if (cc[u] != 0xffffffffu) sp_verify(bitmap, cc[u]);
         __syncthreads();
-        SP_AT(4);
+        nx.at(4);
         if (!NUMERIC) {
-          int cnt = (uint32_t)tid < NCH ? sp_count_clear_chunk(bitmap, lw) : 0;
-#pragma unroll
-          for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-          if (lane == 0 && cnt) atomicAdd(reinterpret_cast<unsigned long long*>(p.counts + i), (unsigned long long)cnt);
+          sp_store_count(p, i, (uint32_t)tid < NCH ? sp_count_clear_chunk(bitmap, lw) : 0);
           break;  // the next row's staging barriers order the clears before its marks
         }
         const int wc = sp_scan<true>(bitmap, pre4, tbase, tflag, lw, NCH, s_warp);
@@ -427,7 +529,7 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
         // row is still ranking its products
         if (FUSED && tid == 0) sp_st_status(p.status + i, kStAgg | (unsigned long long)wc);
         __syncthreads();
-        SP_AT(5);
+        nx.at(5);
         // rank; every product writes (its id, its column) into the slot: the last writer owns the slot
 #pragma unroll
         for (int u = 0; u < kFlatU; u++) {
@@ -439,7 +541,7 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
           }
         }
         __syncthreads();
-        SP_AT(6);
+        nx.at(6);
         uint32_t dmask = 0;
         if (has_val) {
 #pragma unroll
@@ -453,30 +555,16 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
             }
           }
         }
-        if (FUSED && warp == 0 && wc > 0) {
-          // where this row starts in the output: nnz of all earlier rows (decoupled look-back), then publish the
-          // inclusive prefix for the rows behind
-          const int64_t base = sp_lookback(p.status, i, lane, p.dbg);
-          if (lane == 0) {
-            sp_st_status(p.status + i, kStPrefix | (unsigned long long)(base + wc));
-            s_base = base;
-          }
-        }
+        if (FUSED && warp == 0 && wc > 0) sp_place(p, i, wc, lane, s_base);
         if (__syncthreads_or(dmask != 0)) {
 #pragma unroll
           for (int u = 0; u < kFlatU; u++)
             if (dmask & (1u << u)) atomicAdd(&acc[cc[u] >> kMaxWindowLog2], pv[u]);
           __syncthreads();
         }
-        SP_AT(7);
-        int64_t ob;
-        if (FUSED) ob = s_base;
-        else ob = p.rowptr_c[i];
-        int nw = wc;
-        if (FUSED && wc > 0 && ob + wc > p.capacity) {  // cannot happen with capacity >= sum of products; never write past it
-          nw = 0;
-          if (tid == 0) *p.overflow = 1;
-        }
+        nx.at(7);
+        const int64_t ob = FUSED ? s_base : p.rowptr_c[i];
+        const int nw = (FUSED && ob < 0) ? 0 : wc;  // a row that does not fit writes nothing
         for (int q = tid; q < nw; q += kSpThreads) {
           __stcs(p.col_c + ob + q, (int64_t)(scol[q] & (uint32_t)(kMaxWindowBits - 1)));
           if (p.row_c) __stcs(p.row_c + ob + q, i);
@@ -489,7 +577,7 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
       }
 
       // ================= general row: products re-walked per pass, window by window =================
-      SP_AT(2);
+      nx.at(2);
       int64_t win_lo = 0, win_hi = 0;  // window index range [win_lo, win_hi]
       if (multi_window) {
         // B rows are column-sorted (SparseStorage invariant): first/last entry bound the row's columns
@@ -510,103 +598,40 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
         else { win_lo = s_min / W; win_hi = s_max / W; }
         __syncthreads();
       }
-      const bool single_batch = n_a <= kABatch;
+      const SpWalk<NUMERIC, T> walk{p, a_s, a_e, n_a <= kABatch, s_bs, s_len, s_av, pol_b};
       int64_t done = 0;  // nnz of this row emitted by previous windows
       int64_t out0 = 0;
       if (MODE == SP_NUM) out0 = p.rowptr_c[i];
-      int cnt = 0;       // symbolic: columns this thread was first on
-
-      // walk every product of the row that falls into [wlo, whi); BODY sees c (column), c0 (window-relative),
-      // e (A entry in the staged batch), ebs + f (index into B)
-#define SP_WALK(BODY)                                                              \
-  for (int64_t ab = a_s; ab < a_e; ab += kABatch) {                                \
-    const int na = (int)min((int64_t)kABatch, a_e - ab);                           \
-    if (!single_batch) {                                                           \
-      __syncthreads();                                                             \
-      if (tid < na) {                                                              \
-        const int64_t k = p.col_a[ab + tid];                                       \
-        const int64_t kb = p.rowptr_b[k];                                          \
-        s_bs[tid] = kb;                                                            \
-        s_len[tid] = (int)(p.rowptr_b[k + 1] - kb);                                \
-        if (NUMERIC) s_av[tid] = va ? va[ab + tid] : (T)1;                         \
-      }                                                                            \
-      __syncthreads();                                                             \
-    }                                                                              \
-    for (int e = warp; e < na; e += kSpWarps) {                                    \
-      const int64_t ebs = s_bs[e];                                                 \
-      const int elen = s_len[e];                                                   \
-      for (int f = lane; f < elen; f += 32) {                                      \
-        const int64_t c = (int64_t)ldg64_hint(p.col_b + ebs + f, pol_b);           \
-        if (c >= wlo && c < whi) {                                                 \
-          const uint32_t c0 = (uint32_t)(c - wlo);                                 \
-          BODY                                                                     \
-        }                                                                          \
-      }                                                                            \
-    }                                                                              \
-  }
-      // counting pass (the whole job of the symbolic kernel; in single-pass mode it gives the row's nnz before
-      // anything is written): mark with atomicOr, whose return value tells a product whether it was first
-#define SP_COUNT_PASS()                                                            \
-  for (int64_t win = win_lo; win <= win_hi; win++) {                               \
-    const int64_t wlo = win * W, whi = wlo + W;                                    \
-    SP_WALK({                                                                      \
-      const uint32_t bit = 1u << (c0 & 31u);                                       \
-      const uint32_t old = atomicOr(&bitmap[sp_phys(c0 >> 5)], bit);               \
-      if (!(old & bit)) cnt++;                                                     \
-      tflag[c0 >> (5 + lw)] = 1;                                                   \
-    })                                                                             \
-    __syncthreads();                                                               \
-    if ((uint32_t)tid < NCH && tflag[tid]) {                                       \
-      sp_count_clear_chunk(bitmap, lw);                                            \
-      tflag[tid] = 0;                                                              \
-    }                                                                              \
-    __syncthreads();                                                               \
-  }
 
       if (!NUMERIC) {
-        SP_COUNT_PASS();
-#pragma unroll
-        for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-        if (lane == 0 && cnt) atomicAdd(reinterpret_cast<unsigned long long*>(p.counts + i), (unsigned long long)cnt);
-        SP_AT(3);
+        sp_store_count(p, i, sp_count_pass(walk, win_lo, win_hi, W, bitmap, tflag, lw, NCH));
+        nx.at(3);
         break;
       }
       bool skip_row = false;
       if (FUSED) {
         if (tid == 0) s_total = 0;
         __syncthreads();
-        SP_COUNT_PASS();
-#pragma unroll
-        for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+        const int cnt = sp_warp_sum(sp_count_pass(walk, win_lo, win_hi, W, bitmap, tflag, lw, NCH));
         if (lane == 0 && cnt) atomicAdd(&s_total, cnt);
         __syncthreads();
         const int total = s_total;
         if (warp == 0) {
           if (lane == 0) sp_st_status(p.status + i, kStAgg | (unsigned long long)total);
-          if (total > 0) {
-            const int64_t base = sp_lookback(p.status, i, lane, p.dbg);
-            if (lane == 0) {
-              sp_st_status(p.status + i, kStPrefix | (unsigned long long)(base + total));
-              s_base = base;
-            }
-          }
+          if (total > 0) sp_place(p, i, total, lane, s_base);
         }
         __syncthreads();
         out0 = s_base;
-        if (total == 0) skip_row = true;
-        else if (out0 + total > p.capacity) {
-          skip_row = true;
-          if (tid == 0) *p.overflow = 1;
-        }
+        skip_row = total == 0 || out0 < 0;
       }
       if (!skip_row) {
         for (int64_t win = win_lo; win <= win_hi; win++) {
           const int64_t wlo = win * W, whi = wlo + W;
           // ---- mark ----
-          SP_WALK({
+          walk(wlo, whi, [&](int64_t, uint32_t c0, int, int64_t) {
             atomicOr(&bitmap[sp_phys(c0 >> 5)], 1u << (c0 & 31u));
             tflag[c0 >> (5 + lw)] = 1;
-          })
+          });
           __syncthreads();
           const int wc = sp_scan<false>(bitmap, pre4, tbase, tflag, lw, NCH, s_warp);
           const int64_t ob = out0 + done;
@@ -615,7 +640,7 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
             for (int q = tid; q < wc; q += kSpThreads) val_c[ob + q] = (T)0;
           __syncthreads();
           // ---- rank every product: column (same-value races are benign), value via L2 atomics ----
-          SP_WALK({
+          walk(wlo, whi, [&](int64_t c, uint32_t c0, int e, int64_t b) {
             const uint32_t r = sp_rank<false>(bitmap, pre4, tbase, lw, c0);
             if (staged) {
               scol[r] = c0;
@@ -623,8 +648,8 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
               p.col_c[ob + r] = c;
               if (p.row_c) p.row_c[ob + r] = i;
             }
-            if (has_val) atomicAdd(val_c + ob + r, s_av[e] * (vb ? ldg_hint(vb + ebs + f, pol_b) : (T)1));
-          })
+            if (has_val) atomicAdd(val_c + ob + r, s_av[e] * (vb ? ldg_hint(vb + b, pol_b) : (T)1));
+          });
           __syncthreads();
           if (staged) {
             for (int q = tid; q < wc; q += kSpThreads) {
@@ -641,27 +666,12 @@ __global__ void __launch_bounds__(kSpThreads, MODE == SP_SYM ? 5 : (sizeof(T) ==
           __syncthreads();
         }
       }
-#undef SP_WALK
-#undef SP_COUNT_PASS
-      SP_AT(3);
+      nx.at(3);
     } while (false);
-    // whatever part of the next-row schedule this row's path did not reach: the ticket and the row extent are
-    // mandatory, the metadata prefetch is optional (a row without it loads its metadata at its start)
-    if (stage == 0) {
-      if (tid == 0) s_claim[par ^ 1] = atomicAdd(p.counter, 1u);
-      stage = 1;
-    }
-    if (stage == 1) {
-      __syncthreads();
-      SP_NEXT_ROW();
-    }
-#undef SP_AT
-#undef SP_PF_STAGE1
-#undef SP_PF_STAGE2
-#undef SP_NEXT_ROW
-    i = nrow;
-    a_s = nx_s;
-    a_e = nx_e;
+    nx.finish();
+    i = nx.row;
+    a_s = nx.s;
+    a_e = nx.e;
     par ^= 1;
   }
 }
@@ -691,10 +701,10 @@ __global__ void __launch_bounds__(256) sp_bound_kernel(const int64_t* __restrict
   if ((threadIdx.x & 31) == 0 && s) atomicAdd(out, s);
 }
 
-__global__ void sp_copy_last_kernel(const int64_t* rowptr_c, int64_t M, int64_t* nnz_dev) { *nnz_dev = rowptr_c[M]; }
-// nnz(C), or -1 when a row did not fit into the caller's arrays (nothing was written past them)
-__global__ void sp_finish_fused_kernel(const int64_t* rowptr_c, int64_t M, const int* overflow, int64_t* nnz_dev) {
-  *nnz_dev = *overflow ? (int64_t)-1 : rowptr_c[M];
+// nnz(C) = rowptr_c[M], or -1 when the single pass raised `overflow` (a row did not fit into the caller's arrays;
+// nothing was written past them)
+__global__ void sp_finish_kernel(const int64_t* rowptr_c, int64_t M, const int* overflow, int64_t* nnz_dev) {
+  *nnz_dev = (overflow && *overflow) ? (int64_t)-1 : rowptr_c[M];
 }
 
 static int window_bits_for(int64_t N) {
@@ -716,11 +726,15 @@ static size_t sp_smem_bytes(int window_bits, bool numeric, size_t elem) {
   return b;
 }
 
-struct SpLayout { size_t scalars, status, cub, total, cub_bytes; };
+struct SpLayout {
+  // the scalar block at `scalars`: row ticket (uint32), nnz(C) (int64), product bound (int64), overflow flag (int32)
+  static constexpr size_t kTicket = 0, kNnz = 16, kBound = 32, kOverflow = 48, kScalarBytes = 256;
+  size_t scalars, status, cub, total, cub_bytes;
+};
 static SpLayout sp_layout(int64_t M) {
   SpLayout L;
   size_t off = 0;
-  L.scalars = off; off += 256;
+  L.scalars = off; off += SpLayout::kScalarBytes;
   L.status = off; off += align_up((size_t)(M > 0 ? M : 1) * 8, 256);
   size_t tb = 0, tb2 = 0;
   cub::DeviceScan::InclusiveSum(nullptr, tb, (const int64_t*)nullptr, (int64_t*)nullptr, (int)(M > 0 ? M : 1),
@@ -731,6 +745,19 @@ static SpLayout sp_layout(int64_t M) {
   L.cub = off; off += align_up(L.cub_bytes, 256);
   L.total = off;
   return L;
+}
+
+// what every kernel mode reads: the operands, the row ticket, the window and the scan-chunk width
+static SpParams sp_bind(const int64_t* rowptr_a, const int64_t* col_a, const void* val_a, const int64_t* rowptr_b,
+                        const int64_t* col_b, const void* val_b, int64_t M, int64_t N, char* scalars) {
+  SpParams p{};
+  p.rowptr_a = rowptr_a; p.col_a = col_a; p.val_a = val_a;
+  p.rowptr_b = rowptr_b; p.col_b = col_b; p.val_b = val_b;
+  p.M = M; p.N = N;
+  p.counter = (unsigned int*)(scalars + SpLayout::kTicket);
+  p.window_bits = window_bits_for(N);
+  p.log2_wpt = log2_wpt_for(p.window_bits);
+  return p;
 }
 
 template <int MODE, typename T> static int sp_launch(const SpParams& p, cudaStream_t st) {
@@ -770,28 +797,21 @@ extern "C" int tsb200_spspmm_symbolic(const int64_t* rowptr_a, const int64_t* co
   const SpLayout L = sp_layout(M);
   if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
   char* ws = (char*)workspace;
-  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, 256, st));
+  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, SpLayout::kScalarBytes, st));
   TSB_CUDA_TRY(cudaMemsetAsync(rowptr_c, 0, (size_t)(M + 1) * 8, st));
   if (M == 0 || nnz_a == 0 || nnz_b == 0) {
     if (nnz_c_host) *nnz_c_host = 0;
     return 0;
   }
   if (!rowptr_a || !col_a || !rowptr_b || !col_b) return TSB200_ERR_INVALID_ARG;
-  SpParams p;
-  p.rowptr_a = rowptr_a; p.col_a = col_a; p.val_a = nullptr;
-  p.rowptr_b = rowptr_b; p.col_b = col_b; p.val_b = nullptr;
-  p.M = M; p.Kd = Kd; p.N = N;
-  p.counts = rowptr_c + 1; p.rowptr_c = nullptr; p.row_c = nullptr; p.col_c = nullptr; p.val_c = nullptr;
-  p.counter = (unsigned int*)(ws + L.scalars);
-  p.window_bits = window_bits_for(N);
-  p.log2_wpt = log2_wpt_for(p.window_bits);
-  p.status = nullptr; p.capacity = 0; p.overflow = nullptr; p.dbg = nullptr; p.claim_slot = 0;
+  SpParams p = sp_bind(rowptr_a, col_a, nullptr, rowptr_b, col_b, nullptr, M, N, ws + L.scalars);
+  p.counts = rowptr_c + 1;
   int rc = sp_launch<SP_SYM, float>(p, st);
   if (rc) return rc;
   size_t tb = L.cub_bytes;
   TSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(ws + L.cub, tb, rowptr_c + 1, rowptr_c + 1, (int)M, st));
-  int64_t* nnz_dev = (int64_t*)(ws + L.scalars + 16);
-  sp_copy_last_kernel<<<1, 1, 0, st>>>(rowptr_c, M, nnz_dev);
+  int64_t* nnz_dev = (int64_t*)(ws + L.scalars + SpLayout::kNnz);
+  sp_finish_kernel<<<1, 1, 0, st>>>(rowptr_c, M, nullptr, nnz_dev);
   TSB_LAUNCH_CHECK();
   if (nnz_c_host) TSB_CUDA_TRY(cudaMemcpyAsync(nnz_c_host, nnz_dev, 8, cudaMemcpyDeviceToHost, st));
   return 0;
@@ -810,16 +830,9 @@ extern "C" int tsb200_spspmm_numeric(const int64_t* rowptr_a, const int64_t* col
   const SpLayout L = sp_layout(M);
   if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
   char* ws = (char*)workspace;
-  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, 256, st));
-  SpParams p;
-  p.rowptr_a = rowptr_a; p.col_a = col_a; p.val_a = val_a;
-  p.rowptr_b = rowptr_b; p.col_b = col_b; p.val_b = val_b;
-  p.M = M; p.Kd = Kd; p.N = N;
-  p.counts = nullptr; p.rowptr_c = rowptr_c; p.row_c = row_c; p.col_c = col_c; p.val_c = val_c;
-  p.counter = (unsigned int*)(ws + L.scalars);
-  p.window_bits = window_bits_for(N);
-  p.log2_wpt = log2_wpt_for(p.window_bits);
-  p.status = nullptr; p.capacity = 0; p.overflow = nullptr; p.dbg = nullptr; p.claim_slot = 0;
+  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, SpLayout::kScalarBytes, st));
+  SpParams p = sp_bind(rowptr_a, col_a, val_a, rowptr_b, col_b, val_b, M, N, ws + L.scalars);
+  p.rowptr_c = rowptr_c; p.row_c = row_c; p.col_c = col_c; p.val_c = val_c;
   if (val_c && dtype == TSB200_F64) return sp_launch<SP_NUM, double>(p, st);
   return sp_launch<SP_NUM, float>(p, st);
 }
@@ -827,9 +840,10 @@ extern "C" int tsb200_spspmm_numeric(const int64_t* rowptr_a, const int64_t* col
 extern "C" int tsb200_spspmm_bound(const int64_t* col_a, const int64_t* rowptr_b, int64_t nnz_a, void* workspace,
                                    size_t workspace_bytes, int64_t* bound_host, void* stream) {
   if (nnz_a < 0) return TSB200_ERR_INVALID_ARG;
-  if (!workspace || workspace_bytes < 256) return TSB200_ERR_WORKSPACE;
+  // only the scalar block is used, which sits at the start of every SpSpMM workspace
+  if (!workspace || workspace_bytes < SpLayout::kScalarBytes) return TSB200_ERR_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* d = (unsigned long long*)((char*)workspace + 32);
+  unsigned long long* d = (unsigned long long*)((char*)workspace + SpLayout::kBound);
   TSB_CUDA_TRY(cudaMemsetAsync(d, 0, 8, st));
   if (nnz_a > 0) {
     if (!col_a || !rowptr_b) return TSB200_ERR_INVALID_ARG;
@@ -855,38 +869,22 @@ extern "C" int tsb200_spspmm_fused(const int64_t* rowptr_a, const int64_t* col_a
   const SpLayout L = sp_layout(M);
   if (!workspace || workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
   char* ws = (char*)workspace;
-  // scalars: [0] row ticket, [16] nnz(C) (int64), [32] product bound (tsb200_spspmm_bound), [48] overflow flag
-  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, 32, st));
-  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars + 48, 0, 8, st));
+  // the ticket and nnz(C), then the overflow flag; the product bound stays
+  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars, 0, SpLayout::kBound, st));
+  TSB_CUDA_TRY(cudaMemsetAsync(ws + L.scalars + SpLayout::kOverflow, 0, 8, st));
   TSB_CUDA_TRY(cudaMemsetAsync(rowptr_c, 0, (size_t)(M + 1) * 8, st));
-  int64_t* nnz_dev = (int64_t*)(ws + L.scalars + 16);
   if (M == 0 || nnz_a == 0 || nnz_b == 0) {
-    if (nnz_c_host) { nnz_c_host[0] = 0; }
+    if (nnz_c_host) *nnz_c_host = 0;
     return 0;
   }
   if (!rowptr_a || !col_a || !rowptr_b || !col_b || (capacity > 0 && !col_c)) return TSB200_ERR_INVALID_ARG;
   TSB_CUDA_TRY(cudaMemsetAsync(ws + L.status, 0, (size_t)M * 8, st));
-  SpParams p;
-  p.rowptr_a = rowptr_a; p.col_a = col_a; p.val_a = val_a;
-  p.rowptr_b = rowptr_b; p.col_b = col_b; p.val_b = val_b;
-  p.M = M; p.Kd = Kd; p.N = N;
-  p.counts = nullptr; p.rowptr_c = nullptr; p.row_c = row_c; p.col_c = col_c; p.val_c = val_c;
-  p.counter = (unsigned int*)(ws + L.scalars);
+  SpParams p = sp_bind(rowptr_a, col_a, val_a, rowptr_b, col_b, val_b, M, N, ws + L.scalars);
+  p.row_c = row_c; p.col_c = col_c; p.val_c = val_c;
   p.status = (unsigned long long*)(ws + L.status);
   p.capacity = capacity;
-  p.overflow = (int*)(ws + L.scalars + 48);
-  p.dbg = nullptr;
-  p.claim_slot = kClaimSlotDefault;
-  if (const char* ev = getenv("TSB200_SPSPMM_CLAIM")) {  // tuning knob, 0..6
-    const int v = atoi(ev);
-    if (v >= 0 && v <= 6) p.claim_slot = v;
-  }
-  if (getenv("TSB200_SPSPMM_DEBUG")) {  // look-back statistics in scalars [64..88): steps, empty polls, look-backs
-    p.dbg = (unsigned long long*)(ws + L.scalars + 64);
-    TSB_CUDA_TRY(cudaMemsetAsync(p.dbg, 0, 24, st));
-  }
-  p.window_bits = window_bits_for(N);
-  p.log2_wpt = log2_wpt_for(p.window_bits);
+  p.overflow = (int*)(ws + L.scalars + SpLayout::kOverflow);
+  p.claim_slot = kClaimSlot;
   int rc = (val_c && dtype == TSB200_F64) ? sp_launch<SP_FUSED, double>(p, st) : sp_launch<SP_FUSED, float>(p, st);
   if (rc) return rc;
   // rowptr_c[1 + i] = running maximum of the published inclusive prefixes
@@ -897,8 +895,9 @@ extern "C" int tsb200_spspmm_fused(const int64_t* rowptr_a, const int64_t* col_a
   TSB_LAUNCH_CHECK();
   size_t tb = L.cub_bytes;
   TSB_CUDA_TRY(cub::DeviceScan::InclusiveScan(ws + L.cub, tb, rowptr_c + 1, rowptr_c + 1, cub::Max(), (int)M, st));
-  sp_finish_fused_kernel<<<1, 1, 0, st>>>(rowptr_c, M, p.overflow, nnz_dev);
+  sp_finish_kernel<<<1, 1, 0, st>>>(rowptr_c, M, p.overflow, (int64_t*)(ws + L.scalars + SpLayout::kNnz));
   TSB_LAUNCH_CHECK();
-  if (nnz_c_host) TSB_CUDA_TRY(cudaMemcpyAsync(nnz_c_host, nnz_dev, 8, cudaMemcpyDeviceToHost, st));
+  if (nnz_c_host)
+    TSB_CUDA_TRY(cudaMemcpyAsync(nnz_c_host, ws + L.scalars + SpLayout::kNnz, 8, cudaMemcpyDeviceToHost, st));
   return 0;
 }

@@ -853,40 +853,40 @@ def spspmm(rowptr_a: Tensor, col_a: Tensor, val_a: Optional[Tensor], rowptr_b: T
     esize = 0 if not want_value else (8 if dtype == torch.float64 else 4)
     # two_phase (symbolic + numeric kernels) is the default. "fused" selects the single-pass kernel (rows placed by
     # a decoupled look-back, outputs sized by the product bound): bit-identical structure, one kernel instead of two,
-    # kept as an option.
+    # kept as an option. "auto" takes the single pass when the product bound fits comfortably into the memory still
+    # available, otherwise it counts first (two phases).
     mode = os.environ.get("TSB200_SPSPMM", "two_phase")
-    with _on_device(dev):
-        nws = lib.tsb200_spspmm_workspace_bytes(M, Kd, N, nnz_a, nnz_b)
-        ws = _workspace(nws, dev)
-        st = _stream(dev)
+    dt = _dtype_code(dtype) if want_value else 0
+
+    def single_pass():
+        """The product bound, then the single pass into arrays of that size; None when auto declines."""
         pin = _PinnedScalar()
-        if mode in ("fused", "auto"):
-            # single pass: output arrays sized by the number of products (an upper bound of nnz(C)); taken when that
-            # bound fits comfortably into the memory still available, otherwise count first (two phases)
-            check(lib.tsb200_spspmm_bound(_p(col_a), _p(rowptr_b), nnz_a, _p(ws), nws, pin.ptr(), st),
-                  "tsb200_spspmm_bound")
-            torch.cuda.current_stream(dev).synchronize()
-            bound = pin.read()
-            pin = _PinnedScalar()
-            if mode == "fused" or bound * (16 + esize) <= 0.45 * _available_bytes(dev):
-                row_c = torch.empty(bound, dtype=torch.int64, device=dev)
-                col_c = torch.empty(bound, dtype=torch.int64, device=dev)
-                val_c = torch.empty(bound, dtype=dtype, device=dev) if want_value else None
-                check(lib.tsb200_spspmm_fused(_p(rowptr_a), _p(col_a), _p(val_a), _p(rowptr_b), _p(col_b), _p(val_b),
-                                              M, Kd, N, nnz_a, nnz_b, _p(rowptr_c), _p(row_c), _p(col_c), _p(val_c),
-                                              bound, _dtype_code(dtype) if want_value else 0, _p(ws), nws, pin.ptr(),
-                                              st), "tsb200_spspmm_fused")
-                torch.cuda.current_stream(dev).synchronize()
-                nnz_c = pin.read()
-                if nnz_c < 0:  # cannot happen with capacity = number of products
-                    raise _lib.Tsb200Error("tsb200_spspmm_fused: output capacity exceeded")
-                row_c, col_c = row_c[:nnz_c], col_c[:nnz_c]
-                val_c = None if val_c is None else val_c[:nnz_c]
-                if nnz_c < 0.75 * bound:  # many merged products: do not keep the oversized allocations alive
-                    row_c, col_c = row_c.clone(), col_c.clone()
-                    val_c = None if val_c is None else val_c.clone()
-                return rowptr_c, row_c, col_c, val_c
-            pin = _PinnedScalar()
+        check(lib.tsb200_spspmm_bound(_p(col_a), _p(rowptr_b), nnz_a, _p(ws), nws, pin.ptr(), st),
+              "tsb200_spspmm_bound")
+        torch.cuda.current_stream(dev).synchronize()
+        bound = pin.read()
+        if mode == "auto" and bound * (16 + esize) > 0.45 * _available_bytes(dev):
+            return None
+        row_c = torch.empty(bound, dtype=torch.int64, device=dev)
+        col_c = torch.empty(bound, dtype=torch.int64, device=dev)
+        val_c = torch.empty(bound, dtype=dtype, device=dev) if want_value else None
+        pin = _PinnedScalar()
+        check(lib.tsb200_spspmm_fused(_p(rowptr_a), _p(col_a), _p(val_a), _p(rowptr_b), _p(col_b), _p(val_b), M, Kd,
+                                      N, nnz_a, nnz_b, _p(rowptr_c), _p(row_c), _p(col_c), _p(val_c), bound, dt, _p(ws),
+                                      nws, pin.ptr(), st), "tsb200_spspmm_fused")
+        torch.cuda.current_stream(dev).synchronize()
+        nnz_c = pin.read()
+        if nnz_c < 0:  # cannot happen with capacity = number of products
+            raise _lib.Tsb200Error("tsb200_spspmm_fused: output capacity exceeded")
+        row_c, col_c = row_c[:nnz_c], col_c[:nnz_c]
+        val_c = None if val_c is None else val_c[:nnz_c]
+        if nnz_c < 0.75 * bound:  # many merged products: do not keep the oversized allocations alive
+            row_c, col_c = row_c.clone(), col_c.clone()
+            val_c = None if val_c is None else val_c.clone()
+        return rowptr_c, row_c, col_c, val_c
+
+    def two_phase():
+        pin = _PinnedScalar()
         check(lib.tsb200_spspmm_symbolic(_p(rowptr_a), _p(col_a), _p(rowptr_b), _p(col_b), M, Kd, N, nnz_a,
                                          nnz_b, _p(rowptr_c), _p(ws), nws, pin.ptr(), st),
               "tsb200_spspmm_symbolic")
@@ -898,9 +898,15 @@ def spspmm(rowptr_a: Tensor, col_a: Tensor, val_a: Optional[Tensor], rowptr_b: T
         if nnz_c > 0:
             check(lib.tsb200_spspmm_numeric(_p(rowptr_a), _p(col_a), _p(val_a), _p(rowptr_b), _p(col_b),
                                             _p(val_b), M, Kd, N, nnz_a, nnz_b, _p(rowptr_c), _p(row_c),
-                                            _p(col_c), _p(val_c), _dtype_code(dtype) if want_value else 0,
-                                            _p(ws), nws, st), "tsb200_spspmm_numeric")
-    return rowptr_c, row_c, col_c, val_c
+                                            _p(col_c), _p(val_c), dt, _p(ws), nws, st), "tsb200_spspmm_numeric")
+        return rowptr_c, row_c, col_c, val_c
+
+    with _on_device(dev):
+        nws = lib.tsb200_spspmm_workspace_bytes(M, Kd, N, nnz_a, nnz_b)
+        ws = _workspace(nws, dev)
+        st = _stream(dev)
+        out = single_pass() if mode in ("fused", "auto") else None
+        return out if out is not None else two_phase()
 
 
 def _available_bytes(dev: torch.device) -> int:

@@ -510,31 +510,11 @@ def test_bound_loops_over_a_large_a():
     assert int(h) == int(deg[ca].sum())
 
 
-@pytest.mark.parametrize("N", [6000, 3 * MAX_WINDOW + 5])
-def test_claim_slots(oracle, monkeypatch, N):
-    """Single pass with the next row's ticket taken at each schedule slot 0..6 (TSB200_SPSPMM_CLAIM, read per call):
-    the structure and the quantized values of the two-phase run, bit for bit."""
-    case = structured(N)
-    dtype = torch.float32
-    va, vb = quantized_values(case.nnz_a, dtype, 3).to(DEV), quantized_values(case.nnz_b, dtype, 5).to(DEV)
-    ref = call_two_phase(case, va, vb, dtype)
-    check_structure(oracle, case, ref, f"N={N} two-phase")
-    where = _where(case, ref[2])
-    for slot in range(7):
-        monkeypatch.setenv("TSB200_SPSPMM_CLAIM", str(slot))
-        out = call_fused(case, va, vb, dtype)
-        what = f"N={N} claim slot {slot}"
-        assert out[0] == ref[0] and torch.equal(out[1], ref[1]) and torch.equal(out[3], ref[3]), what
-        assert torch.equal(out[2], ref[2]), what
-        assert_bits_equal(out[4], ref[4], where, what)
-
-
-def test_lookback_walks_many_steps(oracle, monkeypatch):
+def test_lookback_across_rows_without_output(oracle):
     """A tall matrix whose rows mostly produce 0 or 1 entries, with runs of 40, 100 and 1000 rows without output and
-    the first row with output at index >= 64. Rows without output never publish a prefix, so a row's look-back must
-    walk (distance to the previous row with output) / 32 steps at least; the debug counters (workspace bytes
-    [64, 88): steps, empty polls, look-backs) show that the multi-step walk ran."""
-    monkeypatch.setenv("TSB200_SPSPMM_DEBUG", "1")
+    the first row with output at index >= 64. Rows without output never publish a prefix, so a row only finds its
+    offset by walking back (distance to the previous row with output) / 32 steps at least: a correct rowptr_c shows
+    that the multi-step walks ran."""
     g = torch.Generator().manual_seed(12)
     M, N = 300_000, 64
     brows = [[], [5], [7, 9]]                     # B row 0 is empty: an A row on it is not empty but has no output
@@ -554,17 +534,43 @@ def test_lookback_walks_many_steps(oracle, monkeypatch):
                                    case.nnz_b, _vp(rpc.t), _vp(rowc.t), _vp(colc.t), None, bound, 0, _vp(ws), nws,
                                    _vp(h), _stream()) == 0
     torch.cuda.synchronize()
-    steps, polls, lookbacks = ws[64:88].view(torch.int64).tolist()
     rp, _, col, _ = oracle.spspmm(case.rpa, case.ca, None, case.rpb, case.cb, None, M, case.Kd, N, False)
     nnz = int(h)
     assert nnz == col.numel() and torch.equal(rpc.t.cpu(), rp) and torch.equal(colc.t[:nnz].cpu(), col)
     out_rows = ((rp[1:] - rp[:-1]) > 0).nonzero().view(-1)
     assert int(out_rows[0]) >= 64
-    assert lookbacks == out_rows.numel()
     prev = torch.cat([torch.tensor([-1]), out_rows[:-1]])
     need = torch.where(prev < 0, (out_rows + 31) // 32, (out_rows - prev + 31) // 32)
     assert int(need.sum()) > out_rows.numel() + 1000 // 32, "the input forces no multi-step walk"
-    assert steps >= int(need.sum()), (steps, int(need.sum()), lookbacks, polls)
+
+
+def test_null_operands_after_the_memsets():
+    """The symbolic and single-pass entry points zero rowptr_c and their scalars before they check the operands (the
+    checks the CPU table cannot reach): a NULL operand, or a NULL col_c with room for output, returns -1 and leaves
+    rowptr_c all zeros."""
+    case = structured(3000)
+    ws, nws = _workspace(case)
+    rp = torch.empty(case.M + 1, dtype=torch.long, device=DEV)
+    col = torch.empty(16, dtype=torch.long, device=DEV)
+    sizes = (case.M, case.Kd, case.N, case.nnz_a, case.nnz_b)
+
+    def symbolic(rpa, ca, rpb, cb, col_c):
+        return lib.tsb200_spspmm_symbolic(rpa, ca, rpb, cb, *sizes, _vp(rp), _vp(ws), nws, None, _stream())
+
+    def fused(rpa, ca, rpb, cb, col_c):
+        return lib.tsb200_spspmm_fused(rpa, ca, None, rpb, cb, None, *sizes, _vp(rp), None, col_c, None, 16, 0, _vp(ws),
+                                       nws, None, _stream())
+
+    good = [_vp(t) for t in case.dev] + [_vp(col)]
+    calls = [(fn, j) for fn in (symbolic, fused) for j in range(4)] + [(fused, 4)]
+    for fn, j in calls:
+        args = list(good)
+        args[j] = None
+        what = f"{fn.__name__}: {['rowptr_a', 'col_a', 'rowptr_b', 'col_b', 'col_c'][j]} = NULL"
+        rp.fill_(SENTINEL)
+        assert fn(*args) == -1, what
+        torch.cuda.synchronize()
+        assert bool((rp == 0).all()), what + ": rowptr_c not zeroed"
 
 
 # ---- edge extents through ops.spspmm ------------------------------------------------------------------------------------

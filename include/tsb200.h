@@ -185,6 +185,31 @@ TSB200_API int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col,
                                       int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * SpMM with a residual added in the store epilogue: out = A x + s * r, for propagation layers with a dense term
+ * (APPNP, GCNII, GIN, residual connections, GCN self-loops as a per-row scale 1/d) without a second pass over the
+ * result (no counterpart in the reference).  B = 1, SUM / MEAN only.
+ *   Let y[m,k] be the fp32 (fp64 for F64) row result tsb200_spmm_fw / tsb200_spmm_fw_planned computes with the same
+ *   arguments, on the same path: after the mean's division, +0 on an empty row. With s = res_scale[m * res_scale_stride]
+ *   (res_scale_stride 0 or 1; float32, or float64 when dtype is F64):
+ *     out[m,k] = round_dtype(fl(y[m,k] + fl(s * res[m,k])))   (one IEEE product and one IEEE add, no FMA contraction)
+ *   rounded to nearest even. NaN and +-inf propagate as IEEE says; a -0 residual on an empty row gives +0.
+ *   dtype F32 / F64 / F16 / BF16; res dtype[M, K] contiguous; value dtype[E] or NULL (1). E == 0: round(fl(+0 + s*r)).
+ *   plan == NULL: workspace tsb200_spmm_fw_workspace_bytes(1, M, K, E, dtype, reduce). Otherwise `plan` is a
+ *   tsb200_spmm_plan of rowptr with its counts, workspace tsb200_spmm_fw_planned_workspace_bytes(K, n_long, n_slot,
+ *   reduce). Both are read on the vector path only (F32 / F16 / BF16, K * sizeof(dtype) % 16 == 0, the alignments of
+ *   tsb200_spmm_fw and a 16-byte aligned res) with E > 0; any other call reads neither. With E == 0 on the vector
+ *   path's conditions a residual-only kernel writes round(fl(+0 + s*r)) in one pass without reading rowptr (the
+ *   residual's gradient s * g is formed this way); otherwise the generic kernel runs and reads rowptr.
+ *   res == NULL: TSB200_ERR_INVALID_ARG (without a residual the call is tsb200_spmm_fw / _planned).
+ *   TSB200_ERR_UNSUPPORTED for MIN / MAX, an integer dtype, or a res_scale not aligned to its element size.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API int tsb200_spmm_fw_res(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                  const void* res, const void* res_scale, int64_t res_scale_stride, void* out,
+                                  int64_t M, int64_t N, int64_t K, int64_t E, int dtype, int reduce, const void* plan,
+                                  size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * FP8 (e4m3) quantisation of a float matrix: the operand of tsb200_spmm_fw_fp8, made without float temporaries (no
  * counterpart in the reference).
  *   x dtype[N, K] with dtype in {F32, F16, BF16}, row m at x + m * ld elements (ld >= K; the last dimension is

@@ -66,9 +66,10 @@ struct SpmmParams {
   uint32_t scale_stride;
   // e4m3 result (tsb200_spmm_fw_fp8_quant): `out` is e4m3 [M, K], out_scale[m] = amax_k |y[m,k]| / 448 (1 if not > 0)
   float* out_scale;
-  // residual (tsb200_spmm_fw_fp8_res, RES kernels): row m of the result is y[m] + fl32(res_scale[m * res_stride] *
-  // res8[m]), res8 e4m3 [M, K], added after the mean's division and before the e4m3 quantisation
-  const uint8_t* res8;
+  // residual (RES kernels; tsb200_spmm_fw_fp8_res, tsb200_spmm_fw_res): row m of the result is y[m] +
+  // fl32(res_scale[m * res_stride] * res[m]), res [M, K] of the dense operand's element type (e4m3 or T), added after
+  // the mean's division and before the e4m3 quantisation
+  const void* res;
   const float* res_scale;
   uint32_t res_stride;
   // multi-head operands (tsb200_spmm_heads / tsb200_sddmm_heads, HEADS kernels only): K = heads * D, and the weight of
@@ -338,26 +339,42 @@ __device__ __forceinline__ uint4 e4m3_pack16(const float* f, float s) {
   return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// ---- e4m3 residual (tsb200_spmm_fw_fp8_res) -------------------------------------------------------------------------
-// z = fl32(y + fl32(rs * r)): one IEEE product and one IEEE add, never contracted to an FMA. The residual is read once,
-// so it is loaded with the streaming (evict-first) hint.
+// ---- residual (tsb200_spmm_fw_fp8_res, tsb200_spmm_fw_res) ---------------------------------------------------------
+// z = fl(y + fl(rs * r)) in the accumulator type (fp32, fp64 for fp64): one IEEE product and one IEEE add, never
+// contracted to an FMA. The residual R has the dense operand's element type: e4m3 (stored as bytes, with its own
+// per-row scale) or the result type T. It is read once, so it is loaded with the streaming (evict-first) hint.
 __device__ __forceinline__ float e4m3_to_f32(uint8_t b) {
   uint32_t r;
   asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)b));
   return __half2float(__ushort_as_half((unsigned short)(r & 0xffffu)));
 }
-__device__ __forceinline__ float res_add(float y, float rs, uint8_t r) {
-  return __fadd_rn(y, __fmul_rn(rs, e4m3_to_f32(r)));
+template <typename R> struct ResElem {  // storage and exact widening of one residual element
+  using raw = R;
+  static __device__ __forceinline__ typename Traits<R>::acc_t widen(R r) { return Traits<R>::to_acc(r); }
+};
+template <> struct ResElem<__nv_fp8_e4m3> {
+  using raw = uint8_t;
+  static __device__ __forceinline__ float widen(uint8_t r) { return e4m3_to_f32(r); }
+};
+template <typename A> __device__ __forceinline__ A res_add(A y, A rs, A r) {
+  if constexpr (std::is_same<A, double>::value) return __dadd_rn(y, __dmul_rn(rs, r));
+  else return __fadd_rn(y, __fmul_rn(rs, r));
 }
-// 16 consecutive results of one lane plus their 16 residual columns (one 16-byte load)
-__device__ __forceinline__ void res_add16(float* f, const uint8_t* r, float rs) {
-  float q[16];
-  Vec<__nv_fp8_e4m3>::unpack(__ldcs(reinterpret_cast<const uint4*>(r)), q);
+// one lane's Vec<R>::VEC consecutive fp32 results plus their residual columns (one 16-byte load)
+template <typename R> __device__ __forceinline__ void res_add_vec(float* f, const typename ResElem<R>::raw* r, float rs) {
+  float q[Vec<R>::VEC];
+  Vec<R>::unpack(__ldcs(reinterpret_cast<const uint4*>(r)), q);
 #pragma unroll
-  for (int i = 0; i < 16; i++) f[i] = __fadd_rn(f[i], __fmul_rn(rs, q[i]));
+  for (int i = 0; i < Vec<R>::VEC; i++) f[i] = res_add(f[i], rs, q[i]);
 }
-__device__ __forceinline__ const uint8_t* res_row(const SpmmParams& p, int64_t row) {
-  return p.res8 + row * p.K + p.k0;
+// the residual row at this launch's first column (the row stores); res_at: one element (the combines)
+template <typename R> __device__ __forceinline__ const typename ResElem<R>::raw* res_row(const SpmmParams& p,
+                                                                                        int64_t row) {
+  return (const typename ResElem<R>::raw*)p.res + row * p.K + p.k0;
+}
+template <typename R> __device__ __forceinline__ const typename ResElem<R>::raw* res_at(const SpmmParams& p, int64_t row,
+                                                                                       int64_t k) {
+  return (const typename ResElem<R>::raw*)p.res + row * p.K + k;
 }
 __device__ __forceinline__ float res_scale(const SpmmParams& p, int64_t row) {
   return __ldg(p.res_scale + row * p.res_stride);

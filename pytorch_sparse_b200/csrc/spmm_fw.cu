@@ -221,14 +221,16 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEAD
     }
   }
 
-  // final write of one row (group 0 lanes). count = row degree. RES: res_row is the row's residual at this launch's
-  // first column and rs its scale; the lane adds its 16 residual columns per chunk after the mean's division.
+  // final write of one row (group 0 lanes). count = row degree. RES: res_row is the row's residual (element type X)
+  // at this launch's first column and rs its scale; the lane adds its VEC residual columns per chunk after the mean's
+  // division.
   template <bool RES = false>
   __device__ __forceinline__ void store_row(T* __restrict__ out_row, int64_t* __restrict__ arg_row,
                                             int64_t count, int64_t E, const bool (&col_ok)[CH], int li,
                                             bool mean, float* __restrict__ part_row = nullptr, int acc_mode = 0,
-                                            const uint8_t* __restrict__ res_row = nullptr, float rs = 0.f) {
-    static_assert(!RES || (Q8 && RED == R_SUM), "residual: fp8 operand, sum / mean");
+                                            const typename ResElem<X>::raw* __restrict__ res_row = nullptr,
+                                            float rs = 0.f) {
+    static_assert(!RES || RED == R_SUM, "residual: sum / mean");
 #pragma unroll
     for (int ch = 0; ch < CH; ch++) {
       if (!col_ok[ch]) continue;
@@ -241,7 +243,7 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEAD
         f[i] = a;
       }
       const int koff = (ch * LPR + li) * VEC;
-      if constexpr (RES) res_add16(f, res_row + koff, rs);
+      if constexpr (RES) res_add_vec<X>(f, res_row + koff, rs);
       if (RED == R_SUM && acc_mode) {  // column-block pipelining: fp32 partial shared by the launches of one product
         float4* pr = reinterpret_cast<float4*>(part_row + koff);
         if (acc_mode != 1) {
@@ -287,7 +289,7 @@ template <typename T, int RED, int LPR, int CH, int U, typename X = T, bool HEAD
         if constexpr (!RES) amax = amax_nan(amax, fabsf(a));
       }
       if constexpr (RES) {
-        res_add16(&acc[ch * VEC], res_row + (ch * LPR + li) * VEC, rs);
+        res_add_vec<X>(&acc[ch * VEC], res_row + (ch * LPR + li) * VEC, rs);
 #pragma unroll
         for (int i = 0; i < VEC; i++) amax = amax_nan(amax, fabsf(acc[ch * VEC + i]));
       }
@@ -469,7 +471,7 @@ template <typename T, int RED, int LPR, int CH, int U> struct MinMax16Engine {
   template <bool RES = false>  // no residual with min / max
   __device__ __forceinline__ void store_row(T* __restrict__ out_row, int64_t* __restrict__ arg_row,
                                             int64_t count, int64_t E, const bool (&col_ok)[CH], int li, bool,
-                                            float* = nullptr, int = 0, const uint8_t* = nullptr, float = 0.f) {
+                                            float* = nullptr, int = 0, const T* = nullptr, float = 0.f) {
     static_assert(!RES, "residual: sum / mean");
 #pragma unroll
     for (int ch = 0; ch < CH; ch++) {
@@ -518,9 +520,9 @@ __device__ __forceinline__ void set_heads(Eng& eng, const SpmmParams& p, const i
 
 // column kk of a multi-segment row (nseg segments, count = its degree): its partials folded in segment order (min/max:
 // the smallest e wins ties), the mean's division applied. CG: read past L1 (partials written by other SMs during the
-// same launch). RES: plus the row's residual (scale rs) in that column. The one definition of the fold: every combine
-// of the SpMM forward calls it.
-template <int RED, bool CG, bool RES = false>
+// same launch). RES: plus the row's residual (element type R, scale rs) in that column. The one definition of the fold:
+// every combine of the SpMM forward calls it.
+template <int RED, bool CG, bool RES = false, typename R = __nv_fp8_e4m3>
 __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow& L, int nseg, int64_t count,
                                              int64_t kk, int64_t& ar, float rs = 0.f) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
@@ -539,13 +541,14 @@ __device__ __forceinline__ float combine_col(const SpmmParams& p, const LongRow&
   }
   ar = r;
   if (RED == R_SUM && p.mean) a = a / (float)(count != 0 ? count : 1);
-  if constexpr (RES) a = res_add(a, rs, __ldcs(p.res8 + L.row_b * p.K + kk));
+  if constexpr (RES) a = res_add(a, rs, ResElem<R>::widen(__ldcs(res_at<R>(p, L.row_b, kk))));
   return a;
 }
 
 // combine the partials of one multi-segment row, in segment order, by ONE WARP (planned mode: the warp that finished
-// the row's last segment); the partials were written by other SMs -> read them past L1. RES: plus the residual.
-template <typename T, int RED, bool RES = false>
+// the row's last segment); the partials were written by other SMs -> read them past L1. RES: plus the residual, of
+// element type R.
+template <typename T, int RED, bool RES = false, typename R = T>
 __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const LongRow& L, int lane, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const int nseg = (int)(L.nseg_count >> 40);
@@ -555,7 +558,7 @@ __device__ __forceinline__ void combine_row_warp(const SpmmParams& p, const Long
     const int64_t kk = p.k0 + k;
     if (kk >= p.K) break;
     int64_t ar;
-    const float a = combine_col<RED, true, RES>(p, L, nseg, count, kk, ar, rs);
+    const float a = combine_col<RED, true, RES, R>(p, L, nseg, count, kk, ar, rs);
     ((T*)p.out)[L.row_b * p.K + kk] = Traits<T>::from_acc(a);
     if (ARG) p.arg_out[L.row_b * p.K + kk] = ar;
   }
@@ -645,7 +648,7 @@ __device__ __forceinline__ void store_partial(const SpmmParams& p, const Eng& en
 // store() is their final row store: the engine's store_row, or store_row_q8 for QO, called by the lanes that hold the
 // row. The segment kernel and the planned drain store a whole-row segment with their own copy of the call: through
 // RowOut the compiler orders their instructions differently (the e4m3-result min/max ones need more registers).
-template <typename T, bool ACC, bool QO, bool RES> struct RowOut {
+template <typename T, bool ACC, bool QO, bool RES, typename X> struct RowOut {
   T* outb;
   int64_t* argb;
   float* partb;
@@ -662,11 +665,11 @@ template <typename T, bool ACC, bool QO, bool RES> struct RowOut {
     if constexpr (QO)
       eng.template store_row_q8<RES>((uint8_t*)p.out + (r0 + rl) * p.K, p.out_scale + r0 + rl,
                                      argb ? argb + (int64_t)rl * p.K : nullptr, count, p.E, col_ok, li, p.mean != 0,
-                                     RES ? res_row(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
+                                     RES ? res_row<X>(p, r0 + rl) : nullptr, RES ? res_scale(p, r0 + rl) : 0.f);
     else
       eng.template store_row<RES>(outb + (int64_t)rl * p.K, argb ? argb + (int64_t)rl * p.K : nullptr, count, p.E,
                                   col_ok, li, p.mean != 0, ACC ? partb + (int64_t)rl * p.K : nullptr,
-                                  ACC ? p.acc_mode : 0, RES ? res_row(p, r0 + rl) : nullptr,
+                                  ACC ? p.acc_mode : 0, RES ? res_row<X>(p, r0 + rl) : nullptr,
                                   RES ? res_scale(p, r0 + rl) : 0.f);
   }
 };
@@ -781,7 +784,7 @@ spmm_vec_kernel(const SpmmParams p) {
     ring.reset(base, __shfl_sync(0xffffffffu, it.rp1, 31));  // lanes >= nrows hold the item's end
     const char* matb = (const char*)p.mat + it.b * p.N * (int64_t)row_bytes + lane_off;
     asm volatile("" : "+l"(matb));  // keep the gather base in a register
-    const RowOut<T, ACC, QO, RES> ro(p, it.b, it.r0);
+    const RowOut<T, ACC, QO, RES, X> ro(p, it.b, it.r0);
 
     for (int rl = 0; rl < it.nrows; rl++) {
       if ((defer_mask >> rl) & 1u) continue;
@@ -814,13 +817,13 @@ spmm_vec_kernel(const SpmmParams p) {
           if (g == 0)
             eng.template store_row_q8<RES>((uint8_t*)p.out + row * p.K, p.out_scale + row,
                                            p.arg_out ? p.arg_out + row * p.K : nullptr, S.end - S.start, p.E, col_ok,
-                                           li, p.mean != 0, RES ? res_row(p, row) : nullptr,
+                                           li, p.mean != 0, RES ? res_row<X>(p, row) : nullptr,
                                            RES ? res_scale(p, row) : 0.f);
         } else {
           if (g == 0)
             eng.template store_row<RES>((T*)p.out + row * p.K + p.k0,
                                         p.arg_out ? p.arg_out + row * p.K + p.k0 : nullptr, S.end - S.start, p.E,
-                                        col_ok, li, p.mean != 0, nullptr, 0, RES ? res_row(p, row) : nullptr,
+                                        col_ok, li, p.mean != 0, nullptr, 0, RES ? res_row<X>(p, row) : nullptr,
                                         RES ? res_scale(p, row) : 0.f);
         }
       } else {
@@ -835,7 +838,7 @@ spmm_vec_kernel(const SpmmParams p) {
         if ((int)finished == (int)(L.nseg_count >> 40) - 1) {
           __threadfence();
           if constexpr (QO) combine_row_warp_q8<RED, RES>(p, L, lane, kcols);
-          else combine_row_warp<T, RED, RES>(p, L, lane, kcols);
+          else combine_row_warp<T, RED, RES, X>(p, L, lane, kcols);
         }
       }
       __syncwarp();
@@ -892,7 +895,7 @@ spmm_gpr_kernel(const SpmmParams p) {
     asm volatile("" : "+l"(matb));
     const int64_t* __restrict__ colb = p.col + base;
     const T* __restrict__ valb = has_val ? (HEADS ? val + base * hstride + hcol[0] : val + base) : nullptr;
-    const RowOut<T, ACC, QO, RES> ro(p, it.b, it.r0);
+    const RowOut<T, ACC, QO, RES, X> ro(p, it.b, it.r0);
     const bool col_ok_arr[1] = {col_ok};
     const int jbase = (int)base;  // absolute nnz index of ring-relative 0 (E < 2^31)
 
@@ -998,14 +1001,14 @@ spmm_seg_kernel(const SpmmParams p) {
         if constexpr (QO)
           eng.template store_row_q8<RES>((uint8_t*)p.out + row * p.K, p.out_scale + row,
                                          p.arg_out ? p.arg_out + row * p.K : nullptr, S.end - S.start, p.E, col_ok,
-                                         li, p.mean != 0, RES ? res_row(p, row) : nullptr,
+                                         li, p.mean != 0, RES ? res_row<X>(p, row) : nullptr,
                                          RES ? res_scale(p, row) : 0.f);
         else
           eng.template store_row<RES>((T*)p.out + (b * p.M + row) * p.K + p.k0,
                                       p.arg_out ? p.arg_out + (b * p.M + row) * p.K + p.k0 : nullptr,
                                       S.end - S.start, p.E, col_ok, li, p.mean != 0,
                                       ACC ? p.partial + (b * p.M + row) * p.K + p.k0 : nullptr, ACC ? p.acc_mode : 0,
-                                      RES ? res_row(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
+                                      RES ? res_row<X>(p, row) : nullptr, RES ? res_scale(p, row) : 0.f);
       } else {
         store_partial<LPR>(p, eng, S.slot, col_ok, li);
       }
@@ -1014,8 +1017,9 @@ spmm_seg_kernel(const SpmmParams p) {
   }
 }
 
-// combine the partials of multi-segment rows, in segment order. RES: plus the residual, after the mean's division.
-template <typename T, int RED, bool RES = false>
+// combine the partials of multi-segment rows, in segment order. RES: plus the residual (element type R), after the
+// mean's division.
+template <typename T, int RED, bool RES = false, typename R = T>
 __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
   const int64_t nlong = p.plan_mask ? p.n_long : min((int64_t)p.counters[2], p.long_cap);
@@ -1028,7 +1032,7 @@ __global__ void spmm_combine_kernel(const SpmmParams p, int kcols) {
       const int64_t kk = p.k0 + k;
       if (kk >= p.K) break;
       int64_t ar;
-      float a = combine_col<RED, false, RES>(p, L, nseg, count, kk, ar, rs);
+      float a = combine_col<RED, false, RES, R>(p, L, nseg, count, kk, ar, rs);
       if (RED == R_SUM && p.acc_mode) {
         float* pr = p.partial + L.row_b * p.K + kk;
         if (p.acc_mode != 1) a += *pr;
@@ -1081,12 +1085,16 @@ __global__ void __launch_bounds__(kCombineThreads) spmm_combine_q8_kernel(const 
 }
 
 // ---- generic fallback: warp per (b,row), lane per column, sequential nnz walk -------------------
-template <typename T, int RED>
+// RES (tsb200_spmm_fw_res, B == 1, sum / mean): plus fl(res_scale[m * res_stride] * res[m, k]) in the accumulator type
+// (res_scale acc_t: float32, float64 for fp64), after the mean's division.
+template <typename T, int RED, bool RES = false>
 __global__ void __launch_bounds__(256)
 spmm_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restrict__ col,
                     const T* __restrict__ value, const T* __restrict__ mat, T* __restrict__ out,
                     int64_t* __restrict__ arg_out, int64_t B, int64_t M, int64_t N, int64_t K,
-                    int64_t E, bool mean) {
+                    int64_t E, bool mean, const T* __restrict__ res = nullptr, const void* __restrict__ res_scale = nullptr,
+                    int64_t res_stride = 0) {
+  static_assert(!RES || RED == R_SUM, "residual: sum / mean");
   const bool HV = value != nullptr;
   using acc_t = typename Traits<T>::acc_t;
   constexpr bool ARG = (RED == R_MIN || RED == R_MAX);
@@ -1128,6 +1136,8 @@ spmm_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restric
       const int64_t cnt = re - rs;
       if (RED == R_SUM && mean) a = a / (acc_t)(cnt > 0 ? cnt : 1);
       if (ARG && cnt == 0) a = (acc_t)0;
+      if constexpr (RES)
+        a = res_add(a, __ldg((const acc_t*)res_scale + m * res_stride), ResElem<T>::widen(__ldcs(res + m * K + k)));
       out[i * K + k] = Traits<T>::from_acc(a);
       if (ARG) arg_out[i * K + k] = cnt > 0 ? ar : E;
     }
@@ -1143,10 +1153,12 @@ static bool vec_eligible(int dtype, int64_t K, int64_t E, int64_t N, const void*
          rowsplit_aligned({mat, out, arg_out}, col, {value});
 }
 
-template <typename T, int RED, bool QO, bool RES = false>
+// R: the residual's element type (X) with a residual, else T, so that every product without one shares a combine kernel
+template <typename T, int RED, bool QO, bool RES, typename X>
 static void launch_combine(const SpmmParams& p, int kcols, cudaStream_t st) {
+  using R = typename std::conditional<RES, X, T>::type;
   if constexpr (QO) spmm_combine_q8_kernel<RED, RES><<<num_sms() * 2, kCombineThreads, 0, st>>>(p, kcols);
-  else spmm_combine_kernel<T, RED, RES><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
+  else spmm_combine_kernel<T, RED, RES, R><<<num_sms() * 2, 128, 0, st>>>(p, kcols);
 }
 
 template <typename T, int RED, bool ACC, int LPR, int CH, int U, int MINB = 1, bool GPR = false, bool PLAN = false,
@@ -1181,13 +1193,13 @@ static int launch_vec(SpmmParams p, cudaStream_t st) {
         kseg<<<grid_seg, kWarpsPerCta * 32, 0, st>>>(p);
         TSB_LAUNCH_CHECK();
         if (p.n_long > 0) {
-          launch_combine<T, RED, QO, RES>(p, kcols, st);
+          launch_combine<T, RED, QO, RES, X>(p, kcols, st);
           TSB_LAUNCH_CHECK();
         }
       }
     } else {
       if (const int rc = launch_rowsplit(kmain, kseg, gc_main, gc_seg, p, st)) return rc;
-      launch_combine<T, RED, QO, RES>(p, kcols, st);
+      launch_combine<T, RED, QO, RES, X>(p, kcols, st);
       TSB_LAUNCH_CHECK();
     }
   }
@@ -1207,7 +1219,11 @@ static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(X);
   const int64_t vecs = p.K / VEC;  // 16-byte vectors per dense row
   // narrow rows: group-per-row kernel (all reductions)
-  constexpr int GB = Q8 ? (MM ? 2 : 3) : 5;
+  // A residual of the operand's type spills every main kernel at the CTAs/SM of its shape (its 16-byte residual chunk
+  // and scale live next to the accumulators), so those take the most CTAs/SM at which none spills: one less, and two
+  // less for the 5-CTA shapes, which still spill at 4 (ptxas table in DESIGN §3.1).
+  constexpr bool FRES = RES && !Q8;
+  constexpr int GB = Q8 ? (MM ? 2 : 3) : (FRES ? 3 : 5);
   if (vecs <= 1) return launch_vec<T, RED, ACC, 1, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
   if (vecs <= 2) return launch_vec<T, RED, ACC, 2, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
   if (vecs <= 4) return launch_vec<T, RED, ACC, 4, 1, 4, GB, true, PLAN, X, QO, RES>(p, st);
@@ -1219,12 +1235,14 @@ static int dispatch_shape(const SpmmParams& p, cudaStream_t st) {
   // A residual (RES) spills the planned kernels of the same shapes at that occupancy, so it takes the QO shapes.
   constexpr bool LOW = MM || QO || RES;
   if (vecs <= 16)
-    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, Q8 && LOW ? 2 : 3, false, PLAN, X, QO, RES>(p, st);
+    return launch_vec<T, RED, ACC, 16, 1, Q8 && !MM ? 4 : 6, (Q8 && LOW) || FRES ? 2 : 3, false, PLAN, X, QO, RES>(p,
+                                                                                                               st);
   if (vecs <= 32)
-    return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (LOW ? 2 : 3) : 5, false, PLAN, X, QO, RES>(p, st);
-  if (vecs <= 64) return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 ? 2 : 3, false, PLAN, X, QO, RES>(p, st);
+    return launch_vec<T, RED, ACC, 32, 1, 4, Q8 ? (LOW ? 2 : 3) : (FRES ? 3 : 5), false, PLAN, X, QO, RES>(p, st);
+  if (vecs <= 64)
+    return launch_vec<T, RED, ACC, 32, 2, Q8 && MM ? 2 : 4, Q8 || FRES ? 2 : 3, false, PLAN, X, QO, RES>(p, st);
   // column-tiled beyond 128 vectors
-  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (LOW ? 1 : 2) : 3, false, PLAN, X, QO, RES>(p, st);
+  return launch_vec<T, RED, ACC, 32, 4, 2, Q8 ? (LOW ? 1 : 2) : (FRES ? 2 : 3), false, PLAN, X, QO, RES>(p, st);
 }
 
 template <typename T, bool PLAN = false, typename X = T, bool QO = false, bool RES = false>
@@ -1547,18 +1565,18 @@ __global__ void __launch_bounds__(256) spmm_res_only_kernel(const SpmmParams p) 
   const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t m = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; m < p.M; m += nw) {
     const float rs = res_scale(p, m);
-    const uint8_t* r = p.res8 + m * p.K;
+    const uint8_t* r = res_at<__nv_fp8_e4m3>(p, m, 0);
     if constexpr (QO) {
       float amax = 0.f;
-      for (int64_t k = lane; k < p.K; k += 32) amax = amax_nan(amax, fabsf(res_add(0.f, rs, __ldcs(r + k))));
+      for (int64_t k = lane; k < p.K; k += 32) amax = amax_nan(amax, fabsf(res_add(0.f, rs, e4m3_to_f32(__ldcs(r + k)))));
 #pragma unroll
       for (int off = 16; off > 0; off >>= 1) amax = amax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, off));
       const float s = e4m3_row_scale(amax);
       if (lane == 0) p.out_scale[m] = s;
-      for (int64_t k = lane; k < p.K; k += 32) ((uint8_t*)p.out)[m * p.K + k] = e4m3_quant(res_add(0.f, rs, r[k]), s);
+      for (int64_t k = lane; k < p.K; k += 32) ((uint8_t*)p.out)[m * p.K + k] = e4m3_quant(res_add(0.f, rs, e4m3_to_f32(r[k])), s);
     } else {
       for (int64_t k = lane; k < p.K; k += 32)
-        ((T*)p.out)[m * p.K + k] = Traits<T>::from_acc(res_add(0.f, rs, __ldcs(r + k)));
+        ((T*)p.out)[m * p.K + k] = Traits<T>::from_acc(res_add(0.f, rs, e4m3_to_f32(__ldcs(r + k))));
     }
   }
 }
@@ -1572,7 +1590,7 @@ static int dispatch_fp8_out(const SpmmParams& p, int out_dtype, int reduce, cuda
 }
 template <bool PLAN, bool QO>
 static int dispatch_fp8_res(const SpmmParams& p, int out_dtype, int reduce, cudaStream_t st) {
-  if (p.res8) return dispatch_fp8_out<PLAN, QO, true>(p, out_dtype, reduce, st);
+  if (p.res) return dispatch_fp8_out<PLAN, QO, true>(p, out_dtype, reduce, st);
   return dispatch_fp8_out<PLAN, QO>(p, out_dtype, reduce, st);
 }
 
@@ -1580,6 +1598,30 @@ template <typename T, bool QO>
 static int launch_res_only(const SpmmParams& p, cudaStream_t st) {
   const int64_t blocks = min((p.M * 32 + 255) / 256, (int64_t)num_sms() * 16);
   spmm_res_only_kernel<T, QO><<<(int)blocks, 256, 0, st>>>(p);
+  TSB_LAUNCH_CHECK();
+  return 0;
+}
+
+// An empty matrix with a residual of the operand's type T, rows of a multiple of 16 bytes (tsb200_spmm_fw_res, E == 0):
+// z = fl32(+0 + fl32(s * r)) rounded once to T, one 16-byte chunk of the residual and of the result per thread and step.
+template <typename T>
+__global__ void __launch_bounds__(256) spmm_res_only_vec_kernel(const SpmmParams p) {
+  constexpr int VEC = Vec<T>::VEC;
+  const int64_t per_row = p.K / VEC, n = p.M * per_row;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t m = i / per_row;
+    float f[VEC];
+#pragma unroll
+    for (int j = 0; j < VEC; j++) f[j] = 0.f;
+    res_add_vec<T>(f, res_at<T>(p, m, (i - m * per_row) * VEC), res_scale(p, m));
+    stg128_stream((T*)p.out + i * VEC, Vec<T>::pack(f));
+  }
+}
+
+template <typename T>
+static int launch_res_only_vec(const SpmmParams& p, cudaStream_t st) {
+  const int64_t chunks = p.M * (p.K / Vec<T>::VEC);
+  spmm_res_only_vec_kernel<T><<<(int)min((chunks + 255) / 256, (int64_t)num_sms() * 16), 256, 0, st>>>(p);
   TSB_LAUNCH_CHECK();
   return 0;
 }
@@ -1606,7 +1648,7 @@ static int spmm_fw_fp8_impl(const int64_t* rowptr, const int64_t* col, const voi
   SpmmParams p{rowptr, col, value, mat, out, arg_out, 1, M, N, K, E};
   p.scale = scale; p.scale_stride = (uint32_t)scale_stride;
   p.out_scale = out_scale;
-  p.res8 = res8; p.res_scale = res_scale; p.res_stride = (uint32_t)res_stride;
+  p.res = res8; p.res_scale = res_scale; p.res_stride = (uint32_t)res_stride;
   if (res8) {
     if (!res_scale || (res_stride != 0 && res_stride != 1)) return TSB200_ERR_INVALID_ARG;
     if (arg) return TSB200_ERR_UNSUPPORTED;
@@ -1676,6 +1718,54 @@ extern "C" int tsb200_spmm_fw_fp8_res(const int64_t* rowptr, const int64_t* col,
                                  out_dtype, reduce, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes,
                                  stream, (const uint8_t*)res8, res_scale, res_scale_stride);
 }
+
+// ---- SpMM with a residual of the operand's type (tsb200_spmm_fw_res) ------------------------------------------------
+// The sum kernels with RES over a T operand (F32 / F16 / BF16 on the vector path, with a 16-byte aligned residual): each
+// storing lane adds the 16-byte chunk of the residual row under its own result chunk. E == 0 on the same condition runs
+// the residual-only vector kernel (also the one-pass s * g of the residual's gradient). Everything else runs the
+// generic kernel with RES, whose +0 sum of an empty row gives the same z = fl(+0 + rho).
+// The definition takes its C linkage from the declaration in tsb200.h (see the guard below).
+int tsb200_spmm_fw_res(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat, const void* res,
+                       const void* res_scale, int64_t res_scale_stride, void* out, int64_t M, int64_t N, int64_t K,
+                       int64_t E, int dtype, int reduce, const void* plan, size_t plan_bytes, int64_t n_seg,
+                       int64_t n_long, int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
+  if (reduce < TSB200_SUM || reduce > TSB200_MAX) return TSB200_ERR_INVALID_ARG;
+  if (dtype_size(dtype) == 0) return TSB200_ERR_INVALID_ARG;
+  if (res_scale_stride != 0 && res_scale_stride != 1) return TSB200_ERR_INVALID_ARG;
+  if (dtype != TSB200_F32 && dtype != TSB200_F64 && dtype != TSB200_F16 && dtype != TSB200_BF16)
+    return TSB200_ERR_UNSUPPORTED;
+  if (reduce == TSB200_MIN || reduce == TSB200_MAX) return TSB200_ERR_UNSUPPORTED;
+  if (M * K == 0) return 0;  // nothing to write
+  if (!rowptr || !out || !res || !res_scale) return TSB200_ERR_INVALID_ARG;
+  if (E > 0 && (!col || !mat)) return TSB200_ERR_INVALID_ARG;
+  if ((uintptr_t)res_scale & (dtype == TSB200_F64 ? 7 : 3)) return TSB200_ERR_UNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+
+  if (vec_eligible(dtype, K, E, N, value, mat, out, col, nullptr) && !((uintptr_t)res & 15)) {
+    SpmmParams p{rowptr, col, value, mat, out, nullptr, 1, M, N, K, E};
+    p.res = res; p.res_scale = (const float*)res_scale; p.res_stride = (uint32_t)res_scale_stride;
+    if (E == 0) return dispatch_vec_dtype(dtype, [&](auto tag) { return launch_res_only_vec<decltype(tag)>(p, st); });
+    if (const int rc = bind_workspace(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, false))
+      return rc;
+    return dispatch_vec_dtype(dtype, [&](auto tag) {
+      using T = decltype(tag);
+      return plan ? dispatch_red_vec<T, true, T, false, true>(p, reduce, st)
+                  : dispatch_red_vec<T, false, T, false, true>(p, reduce, st);
+    });
+  }
+  return dispatch_float_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    spmm_generic_kernel<T, R_SUM, true><<<warp_grid(M, 64), 256, 0, st>>>(
+        rowptr, col, (const T*)value, (const T*)mat, (T*)out, nullptr, 1, M, N, K, E, reduce == TSB200_MEAN,
+        (const T*)res, res_scale, res_scale_stride);
+    TSB_LAUNCH_CHECK();
+    return 0;
+  });
+}
+// Were the definition above ever to drift from the declaration in tsb200.h, it would become a second, C++ overload and
+// the exported C symbol would be left undefined: taking the address of an overload set does not compile.
+[[maybe_unused]] static constexpr auto tsb200_spmm_fw_res_declared_once = &tsb200_spmm_fw_res;
 
 // ---- SpMM with per-head weights (tsb200_spmm_heads) -------------------------------------------------------------
 // The sum kernels with HEADS = true over x [N, H * D]; with value == NULL every weight is 1 and the product is the

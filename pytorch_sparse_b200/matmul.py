@@ -67,7 +67,39 @@ def spmm_max(src: SparseTensor, other: Tensor) -> Tuple[Tensor, Tensor]:
     return torch.ops.tsb200.spmm_max(rowptr, col, value, other)
 
 
-def spmm(src: SparseTensor, other: Tensor, reduce: str = "sum") -> Tensor:
+def spmm_res(src: SparseTensor, other: Tensor, residual: Tensor, residual_scale: Optional[Tensor] = None,
+             reduce: str = "sum") -> Tensor:
+    """`src @ other + residual_scale * residual` in one pass: the residual ([M, K], other's dtype) is added to every row
+    in the kernels' store epilogue, out = round(fl(y + fl(s * r))) with y the fp32 (fp64) sum or mean. `other` is 2-D
+    (bf16, f16, f32, f64); `residual_scale` is None (1) or float32 (float64 for f64) of shape [] or [M]. Differentiable
+    in the values, `other`, `residual` and `residual_scale`; only the caches a requested gradient reads are built."""
+    rowptr, col, value = src.csr()
+    st = src.storage
+    row, rowcount, colptr, csr2csc = st._row, st._rowcount, st._colptr, st._csr2csc
+    row_csc: Optional[Tensor] = None
+    if value is not None:
+        value = value.to(other.dtype)
+        if value.requires_grad:
+            row = st.row()
+    if other.requires_grad:     # A^T @ grad_out runs on the CSC view
+        row = st.row()
+        if reduce == "mean":
+            rowcount = st.rowcount()
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.spmm_res(row, rowptr, col, value, rowcount, colptr, csr2csc, other, row_csc, residual,
+                                     residual_scale, reduce)
+
+
+def spmm(src: SparseTensor, other: Tensor, reduce: str = "sum", residual: Optional[Tensor] = None,
+         residual_scale: Optional[Tensor] = None) -> Tensor:
+    """`src @ other` reduced per row (sum / add / mean / min / max). With `residual` (sum / add / mean, 2-D `other`):
+    `src @ other + residual_scale * residual` in one pass (see `spmm_res`)."""
+    if residual is not None:
+        return spmm_res(src, other, residual, residual_scale, reduce)
+    if residual_scale is not None:
+        raise ValueError("spmm: residual_scale needs a residual")
     if reduce == "sum" or reduce == "add":
         return spmm_sum(src, other)
     elif reduce == "mean":
@@ -276,7 +308,8 @@ def matmul(src, other, reduce="sum"):  # noqa: F811
     raise ValueError("cannot multiply a SparseTensor with this operand")
 
 
-SparseTensor.spmm = lambda self, other, reduce="sum": spmm(self, other, reduce)
+SparseTensor.spmm = lambda self, other, reduce="sum", residual=None, residual_scale=None: spmm(
+    self, other, reduce, residual, residual_scale)
 SparseTensor.spmm_fp8 = lambda self, x8, scale, reduce="sum", out_dtype=torch.bfloat16, residual=None, \
     residual_scale=None: spmm_fp8(self, x8, scale, reduce, out_dtype, residual, residual_scale)
 SparseTensor.spmm_fp8_quant = lambda self, x8, scale, reduce="sum", residual=None, residual_scale=None: spmm_fp8_quant(

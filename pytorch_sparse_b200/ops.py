@@ -220,6 +220,91 @@ def _plan_workspace(plan: Optional[SpmmPlan], plannable: bool, rowptr: Tensor, B
     return pl, _workspace(nws, dev), nws
 
 
+_ONE = {}  # a scalar 1 per (device, dtype): the scale of a residual passed without one
+
+
+def _res_args(what: str, residual: Tensor, residual_scale: Optional[Tensor], mat: Tensor, M: int, red: int):
+    """The checks of the residual of spmm_fw_res; returns (residual_scale, residual_scale_stride)."""
+    _check_cuda(residual, "residual")
+    if red >= 2:
+        raise RuntimeError(f"{what}: a residual is only added to reduce='sum' / 'mean' results, not min / max")
+    if mat.dim() != 2:
+        raise RuntimeError(f"{what}: a residual needs a 2-D dense operand [N, K], got {mat.dim()}-D")
+    if residual.device != mat.device:
+        raise RuntimeError(f"{what}: residual must be on the device of the dense operand ({mat.device})")
+    if residual.dtype != mat.dtype:
+        raise RuntimeError(f"{what}: residual must have the dense operand's dtype {mat.dtype}, got {residual.dtype}")
+    K = mat.size(1)
+    if residual.dim() != 2 or residual.size(0) != M or residual.size(1) != K:
+        raise RuntimeError(f"{what}: residual must have the result's shape [M, K] = [{M}, {K}], "
+                           f"got {list(residual.shape)}")
+    if not residual.is_contiguous():
+        raise RuntimeError(f"{what}: residual must be contiguous")
+    sdt = torch.float64 if mat.dtype == torch.float64 else torch.float32
+    if residual_scale is None:
+        key = (mat.device, sdt)
+        one = _ONE.get(key)
+        if one is None:
+            one = _ONE[key] = torch.ones((), dtype=sdt, device=mat.device)
+        return one, 0
+    _check_cuda(residual_scale, "residual_scale")
+    if residual_scale.device != mat.device:
+        raise RuntimeError(f"{what}: residual_scale must be on the device of the dense operand ({mat.device})")
+    if residual_scale.dtype != sdt:
+        raise RuntimeError(f"{what}: residual_scale must be {sdt} for a {mat.dtype} operand, got {residual_scale.dtype}")
+    if residual_scale.dim() == 0:
+        stride = 0
+    elif residual_scale.dim() == 1 and residual_scale.size(0) == M:
+        stride = 1
+    else:
+        raise RuntimeError(f"{what}: residual_scale must have shape [] or [M] = [{M}], "
+                           f"got {list(residual_scale.shape)}")
+    return residual_scale.contiguous(), stride
+
+
+def spmm_fw_res(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, residual: Tensor,
+                residual_scale: Optional[Tensor] = None, reduce: str = "sum",
+                plan: Optional[SpmmPlan] = None) -> Tensor:
+    """`spmm_fw(rowptr, col, value, mat, reduce)` plus `residual_scale[m] * residual[m]` on every row m, added in the
+    kernels' store epilogue (tsb200_spmm_fw_res): out = round(fl(y + fl(s * r))) with y the fp32 (fp64) row result
+    `spmm_fw` computes on the same path, one IEEE product and one IEEE add. `mat` is 2-D [N, K] (bf16, f16, f32, f64),
+    `residual` [M, K] contiguous in its dtype, `residual_scale` None (1) or float32 (float64 for f64) of shape [] or
+    [M]; reduce sum / add / mean. Planned like `spmm_fw` (the same per-rowptr plan cache). Forward only: see SPMMRes."""
+    _check_cuda(rowptr, "rowptr")
+    _check_cuda(col, "col")
+    if value is not None:
+        _check_cuda(value, "optional_value.value()")
+    _check_cuda(mat, "mat")
+    red = _reduce_code(reduce)
+    M = rowptr.numel() - 1
+    scale, stride = _res_args("spmm_res", residual, residual_scale, mat, M, red)
+    _check_input(rowptr.dim() == 1)
+    _check_input(col.dim() == 1)
+    if value is not None:
+        _check_input(value.dim() == 1)
+        _check_input(value.size(0) == col.size(0))
+        if value.dtype != mat.dtype:
+            raise RuntimeError(f"expected value of dtype {mat.dtype} but got {value.dtype}")
+        value = value.contiguous()
+    rowptr = _i64(rowptr, "rowptr")
+    col = _i64(col, "col")
+    mat = mat.contiguous()
+    dt = _dtype_code(mat.dtype)
+    N, K = mat.shape
+    E = col.numel()
+    dev = mat.device
+    out = torch.empty(M, K, dtype=mat.dtype, device=dev)
+    if out.numel() == 0:
+        return out
+    with _on_device(dev):
+        plannable = E > 0 and dt in (0, 2, 3) and (K * mat.element_size()) % 16 == 0
+        pl, ws, nws = _plan_workspace(plan, plannable, rowptr, 1, M, K, E, dt, red, dev)
+        check(lib.tsb200_spmm_fw_res(_p(rowptr), _p(col), _p(value), _p(mat), _p(residual), _p(scale), stride,
+                                     _p(out), M, N, K, E, dt, red, *pl, _p(ws), nws, _stream(dev)),
+              "tsb200_spmm_fw_res")
+    return out
+
+
 _FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
 
 
@@ -1006,16 +1091,23 @@ class SPMMSum(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         row, rowptr, col, value, colptr, csr2csc, mat, row_csc = ctx.saved_tensors
-        grad_value = grad_mat = None
-        if ctx.has_value and ctx.needs_input_grad[3]:
-            grad_value = spmm_value_bw(row, rowptr, col, mat, grad_out, "sum")
-        if ctx.needs_input_grad[6]:
-            # grad_mat = A^T @ grad_out as a CSR SpMM on the CSC view (csrc/spmm.cpp:100-108)
-            v = value.index_select(0, csr2csc) if ctx.has_value else None
-            if row_csc is None:
-                row_csc = row.index_select(0, csr2csc)
-            grad_mat, _ = spmm_fw(colptr, row_csc, v, grad_out, "sum")
+        grad_value, grad_mat = _sum_grads(ctx.has_value and ctx.needs_input_grad[3], ctx.needs_input_grad[6], row,
+                                          rowptr, col, value, colptr, csr2csc, mat, row_csc, grad_out)
         return None, None, None, grad_value, None, None, grad_mat, None
+
+
+def _sum_grads(need_value: bool, need_mat: bool, row, rowptr, col, value, colptr, csr2csc, mat, row_csc, grad_out):
+    """(grad_value, grad_mat) of a sum SpMM: SPMMSum's backward, shared with SPMMRes."""
+    grad_value = grad_mat = None
+    if need_value:
+        grad_value = spmm_value_bw(row, rowptr, col, mat, grad_out, "sum")
+    if need_mat:
+        # grad_mat = A^T @ grad_out as a CSR SpMM on the CSC view (csrc/spmm.cpp:100-108)
+        v = value.index_select(0, csr2csc) if value is not None else None
+        if row_csc is None:
+            row_csc = row.index_select(0, csr2csc)
+        grad_mat, _ = spmm_fw(colptr, row_csc, v, grad_out, "sum")
+    return grad_value, grad_mat
 
 
 class SPMMMean(torch.autograd.Function):
@@ -1038,20 +1130,86 @@ class SPMMMean(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc = ctx.saved_tensors
-        grad_value = grad_mat = None
-        if ctx.has_value and ctx.needs_input_grad[3]:
-            grad_value = spmm_value_bw(row, rowptr, col, mat, grad_out, "mean")
-        if ctx.needs_input_grad[7]:
-            # per-nnz weight value/count(row) (or 1/count) in CSC order (csrc/spmm.cpp:166-177), divided in the
-            # accumulator type and rounded once to mat's dtype: the forward and grad_value divide by the exact count,
-            # which bf16 (above 256) and f16 (above 2048) cannot always hold (DESIGN §3.2)
-            if row_csc is None:
-                row_csc = row.index_select(0, csr2csc)
-            acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
-            cnt = rowcount.index_select(0, row_csc).to(acc).clamp_(min=1)
-            w = value.index_select(0, csr2csc).to(acc).div_(cnt) if ctx.has_value else cnt.reciprocal_()
-            grad_mat, _ = spmm_fw(colptr, row_csc, w.to(mat.dtype), grad_out, "sum")
+        grad_value, grad_mat = _mean_grads(ctx.has_value and ctx.needs_input_grad[3], ctx.needs_input_grad[7], row,
+                                           rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc, grad_out)
         return None, None, None, grad_value, None, None, None, grad_mat, None
+
+
+def _mean_grads(need_value: bool, need_mat: bool, row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc,
+                grad_out):
+    """(grad_value, grad_mat) of a mean SpMM: SPMMMean's backward, shared with SPMMRes."""
+    grad_value = grad_mat = None
+    if need_value:
+        grad_value = spmm_value_bw(row, rowptr, col, mat, grad_out, "mean")
+    if need_mat:
+        # per-nnz weight value/count(row) (or 1/count) in CSC order (csrc/spmm.cpp:166-177), divided in the
+        # accumulator type and rounded once to mat's dtype: the forward and grad_value divide by the exact count,
+        # which bf16 (above 256) and f16 (above 2048) cannot always hold (DESIGN §3.2)
+        if row_csc is None:
+            row_csc = row.index_select(0, csr2csc)
+        acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
+        cnt = rowcount.index_select(0, row_csc).to(acc).clamp_(min=1)
+        w = value.index_select(0, csr2csc).to(acc).div_(cnt) if value is not None else cnt.reciprocal_()
+        grad_mat, _ = spmm_fw(colptr, row_csc, w.to(mat.dtype), grad_out, "sum")
+    return grad_value, grad_mat
+
+
+_ZERO_PTR = {}  # per device: a zero row pointer, the empty pattern of _scale_rows
+
+
+def _scale_rows(g: Tensor, scale: Tensor) -> Tensor:
+    """s[m] * g[m] in fp32 (fp64), rounded once to g's dtype, in one pass over g (a zero product gives +0): the
+    residual-only SpMM over an empty pattern, tsb200_spmm_fw_res with E = 0 and residual g."""
+    M, K = g.shape
+    z = _ZERO_PTR.get(g.device)
+    if z is None or z.numel() < M + 1:
+        z = _ZERO_PTR[g.device] = torch.zeros(M + 1, dtype=torch.int64, device=g.device)
+    return spmm_fw_res(z[:M + 1], z[:0], None, g.new_empty(0, K), g.contiguous(), scale)
+
+
+class SPMMRes(torch.autograd.Function):
+    """`spmm_fw_res`, sum or mean. grad_value and grad_mat are those of SPMMSum / SPMMMean; grad_residual is
+    s * g formed in fp32 (fp64) and rounded once, in one pass (_scale_rows); grad_residual_scale is sum_k g * r per row
+    ([M]) or over all ([])."""
+    @staticmethod
+    def forward(ctx, row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc, residual, residual_scale,
+                reduce):
+        mean = _reduce_code(reduce) == 1
+        need_value = value is not None and ctx.needs_input_grad[3]
+        need_mat = ctx.needs_input_grad[7]
+        if need_value or need_mat:
+            _assert_present(row, "row")
+        if need_mat:
+            if mean:
+                _assert_present(rowcount, "rowcount")
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+        out = spmm_fw_res(rowptr, col, value, mat, residual, residual_scale, reduce)
+        ctx.mean, ctx.need_value = mean, need_value
+        ctx.save_for_backward(row, rowptr, col, value, rowcount, colptr, csr2csc, mat,
+                              row_csc if need_mat else None, residual if ctx.needs_input_grad[10] else None,
+                              residual_scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc, residual, scale = ctx.saved_tensors
+        need_mat = ctx.needs_input_grad[7]
+        grad_value = grad_mat = grad_res = grad_scale = None
+        if ctx.need_value or need_mat:
+            if ctx.mean:
+                grad_value, grad_mat = _mean_grads(ctx.need_value, need_mat, row, rowptr, col, value, rowcount, colptr,
+                                                   csr2csc, mat, row_csc, grad_out)
+            else:
+                grad_value, grad_mat = _sum_grads(ctx.need_value, need_mat, row, rowptr, col, value, colptr, csr2csc,
+                                                  mat, row_csc, grad_out)
+        acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
+        if ctx.needs_input_grad[9]:
+            grad_res = grad_out if scale is None else _scale_rows(grad_out, scale)
+        if ctx.needs_input_grad[10]:
+            gr = grad_out.to(acc) * residual.to(acc)
+            grad_scale = gr.sum(1) if scale.dim() == 1 else gr.sum()
+        return (None, None, None, grad_value, None, None, None, grad_mat, None, grad_res, grad_scale, None)
 
 
 def _minmax_forward(ctx, reduce, rowptr, col, value, mat):
@@ -1102,6 +1260,13 @@ def spmm_mean(row: Optional[Tensor], rowptr: Tensor, col: Tensor, value: Optiona
               rowcount: Optional[Tensor], colptr: Optional[Tensor], csr2csc: Optional[Tensor],
               mat: Tensor, row_csc: Optional[Tensor] = None) -> Tensor:
     return SPMMMean.apply(row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc)
+
+
+def spmm_res(row: Optional[Tensor], rowptr: Tensor, col: Tensor, value: Optional[Tensor], rowcount: Optional[Tensor],
+             colptr: Optional[Tensor], csr2csc: Optional[Tensor], mat: Tensor, row_csc: Optional[Tensor],
+             residual: Tensor, residual_scale: Optional[Tensor], reduce: str) -> Tensor:
+    return SPMMRes.apply(row, rowptr, col, value, rowcount, colptr, csr2csc, mat, row_csc, residual, residual_scale,
+                         reduce)
 
 
 def spmm_min(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor) -> Tuple[Tensor, Tensor]:

@@ -2,7 +2,7 @@
 (csrc/spmm.cpp:305-348, csrc/convert.cpp:46-48):
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
-    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_fp8, spmm_fp8_quant,
+    torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_res, spmm_fp8, spmm_fp8_quant,
                       quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads, segment_softmax}  (own additions)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
@@ -55,6 +55,10 @@ _EXTRA_SCHEMAS = {
              "Tensor b) -> Tensor",
     "sddmm_fp8": "(Tensor rowptr, Tensor col, Tensor a8, Tensor a_scale, Tensor b8, Tensor b_scale, "
                  "ScalarType out_dtype) -> Tensor",
+    # spmm_sum_csc / spmm_mean_csc (reduce sum, add or mean) plus residual_scale * residual on every row, in one pass
+    "spmm_res": "(Tensor? row, Tensor rowptr, Tensor col, Tensor? value, Tensor? rowcount, Tensor? colptr, "
+                "Tensor? csr2csc, Tensor mat, Tensor? row_csc, Tensor residual, Tensor? residual_scale, str reduce) "
+                "-> Tensor",
     # multi-head: value [E, H] over x [N, H, D]; scores [E, H] of a [M, H, D] and b [N, H, D]
     "spmm_heads": "(Tensor? row, Tensor rowptr, Tensor col, Tensor? value, Tensor? colptr, Tensor? csr2csc, "
                   "Tensor x, Tensor? row_csc) -> Tensor",
@@ -71,7 +75,7 @@ def _csr2csc(row, col, M: int, N: int):
 
 
 _EXTRA_IMPLS = {
-    "spmm_sum_csc": ops.spmm_sum, "spmm_mean_csc": ops.spmm_mean,
+    "spmm_sum_csc": ops.spmm_sum, "spmm_mean_csc": ops.spmm_mean, "spmm_res": ops.spmm_res,
     "coalesce": ops.coalesce, "sort_perm": ops.sort_perm, "csr2csc": _csr2csc,
     "segment_reduce": lambda ptr, value, reduce, perm, seg: ops.segment_reduce(ptr, value, reduce, perm, seg),
     "spspmm": ops.spspmm,

@@ -210,6 +210,35 @@ TSB200_API int tsb200_spmm_fw_res(const int64_t* rowptr, const int64_t* col, con
                                   size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Multi-aggregation SpMM: several per-row aggregations of the messages p_e = value[e] * mat[col[e]] from one gather
+ * pass, for PNA-style layers (no counterpart in the reference).  B = 1.
+ *   aggrs[0..n_aggr) are distinct codes among TSB200_SUM, TSB200_MEAN, TSB200_MIN, TSB200_MAX, TSB200_VAR and
+ *   TSB200_STD (1 <= n_aggr <= 6); out dtype[M, n_aggr, K] holds aggregator aggrs[a] of row m in out[m, a, :].
+ *   SUM, MEAN, MIN, MAX (and arg_min / arg_max): bit for bit what tsb200_spmm_fw / tsb200_spmm_fw_planned returns
+ *   with the same arguments, on the same path and at the same work-item size. With n = max(deg, 1), mu the fp32 (fp64
+ *   for F64) mean and Q = sum_e fma(p_e, p_e, .) accumulated in the sum's order:
+ *     VAR = max(fl(fl(Q / n) - fl(mu * mu)), 0)   (NaN passes)
+ *     STD = sqrt(VAR) where VAR > 1e-5, else 0
+ *   each rounded once to dtype. arg_min / arg_max int64[M, K] or NULL (not stored); each needs its aggregator.
+ *   dtype F32 / F64 / F16 / BF16; value dtype[E] or NULL (1). E == 0: every aggregator 0, args 0.
+ *   plan == NULL: workspace tsb200_spmm_fw_multi_workspace_bytes(K, E, 0, 0, 0). Otherwise `plan` is a tsb200_spmm_plan
+ *   of rowptr with its counts, workspace tsb200_spmm_fw_multi_workspace_bytes(K, E, 1, n_long, n_slot). Both are read
+ *   on the vector path only (F32 / F16 / BF16, K * sizeof(dtype) % 16 == 0, E > 0, the extents and alignments of
+ *   tsb200_spmm_fw, arg_max 16-byte aligned); any other call runs the generic kernel, which reads neither.
+ *   TSB200_ERR_INVALID_ARG for an empty, long, repeating or out-of-range aggrs, or an arg pointer without its aggregator;
+ *   TSB200_ERR_UNSUPPORTED for an integer dtype.
+ * ------------------------------------------------------------------------------------------ */
+#define TSB200_VAR 4
+#define TSB200_STD 5
+TSB200_API size_t tsb200_spmm_fw_multi_workspace_bytes(int64_t K, int64_t E, int planned, int64_t n_long,
+                                                       int64_t n_slot);
+TSB200_API int tsb200_spmm_fw_multi(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                                    const int* aggrs, int n_aggr, void* out, int64_t* arg_min, int64_t* arg_max,
+                                    int64_t M, int64_t N, int64_t K, int64_t E, int dtype, const void* plan,
+                                    size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * FP8 (e4m3) quantisation of a float matrix: the operand of tsb200_spmm_fw_fp8, made without float temporaries (no
  * counterpart in the reference).
  *   x dtype[N, K] with dtype in {F32, F16, BF16}, row m at x + m * ld elements (ld >= K; the last dimension is

@@ -43,6 +43,10 @@ SIGNATURES = {
     "tsb200_spmm_fw_res": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                    c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_void_p, c_size_t,
                                    c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_fw_multi_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int64, c_int64]),
+    "tsb200_spmm_fw_multi": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t,
+                                     c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "tsb200_quantize_fp8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_size_t, c_void_p]),
     "tsb200_spmm_fw_acc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

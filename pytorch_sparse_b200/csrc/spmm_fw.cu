@@ -1429,6 +1429,554 @@ static int launch_generic(const int64_t* rowptr, const int64_t* col, const void*
   return 0;
 }
 
+// ---- multi-aggregation SpMM (tsb200_spmm_fw_multi) -----------------------------------------------------------------
+// One gather pass accumulates, per column, the four statistics every aggregator is formed from: the sum S, the sum of
+// squares Q = sum fma(p, p, .) of the products p, and the min and max of the products rounded to T with their entries.
+// S, min and max follow exactly the single-reduction engines (same lane layout per row width, same per-lane order,
+// butterfly and segment fold), so the sum, mean, min and max slices are spmm's bits. The store epilogue writes only
+// the requested statistics, each into its slice of out [M, A, K], and the args only where their pointer is set.
+enum : int { R_VAR = TSB200_VAR, R_STD = TSB200_STD, kStats = 6 };
+
+struct MultiOut {
+  int64_t* arg_min;  // [M, K] or NULL: not stored
+  int64_t* arg_max;
+  int A;             // slices per row of `out`
+  int8_t slice[kStats];  // slice of each aggregator code, -1 = not requested
+};
+
+// aggregator c of one column from its statistics over a row of `count` entries, in the accumulator type: the mean's
+// IEEE division, var = max(fl(fl(Q / n) - fl(mu * mu)), 0) (no contraction, so a one-entry row gives exactly 0; NaN
+// passes), std = sqrt(var) where var > 1e-5, else 0
+template <typename A>
+__device__ __forceinline__ A multi_stat(int c, A s, A q, A mn, A mx, int64_t count) {
+  const A n = (A)(count > 0 ? count : 1);
+  if (c == R_SUM) return s;
+  if (c == R_MIN) return count == 0 ? (A)0 : mn;
+  if (c == R_MAX) return count == 0 ? (A)0 : mx;
+  const A mu = s / n;
+  if (c == R_MEAN) return mu;
+  A d;
+  if constexpr (std::is_same<A, double>::value) d = __dsub_rn(q / n, __dmul_rn(mu, mu));
+  else d = __fsub_rn(q / n, __fmul_rn(mu, mu));
+  const A var = d < (A)0 ? (A)0 : d;
+  if (c == R_VAR) return var;
+  return var > (A)1e-5 ? sqrt(var) : (A)0;
+}
+
+// the per-lane state of the multi kernels: VEC * CH columns of S, Q, min, max and the two args
+template <typename T, int LPR, int CH, int U> struct MultiEngine {
+  using V = Vec<T>;
+  static constexpr bool Q8 = false;
+  static constexpr int VEC = V::VEC;
+  static constexpr int G = 32 / LPR;
+  static constexpr int NA = VEC * CH;
+
+  float s[NA], q[NA], mn[NA], mx[NA];
+  int amn[NA], amx[NA];
+
+  __device__ __forceinline__ void init() {
+#pragma unroll
+    for (int i = 0; i < NA; i++) {
+      s[i] = 0.f;
+      q[i] = 0.f;
+      mn[i] = Traits<T>::to_acc(Traits<T>::highest());
+      mx[i] = Traits<T>::to_acc(Traits<T>::lowest());
+      amn[i] = amx[i] = 0x7fffffff;
+    }
+  }
+
+  // one gathered vector of one entry (raw value v, entry jabs): the sum as Vec<T>::fma, the min / max on the product
+  // rounded to T as RowEngine::minmax_step (bit for bit the packed 16-bit engine's), Q on the fp32 product
+  __device__ __forceinline__ void step(int ch, typename V::vraw v, const uint4& d, int jabs) {
+    const float vf = V::vfloat(v);
+    float f[VEC];
+    V::unpack(d, f);
+#pragma unroll
+    for (int i = 0; i < VEC; i++) {
+      const int a = ch * VEC + i;
+      s[a] = fmaf(vf, f[i], s[a]);
+      const float pr = __fmul_rn(vf, f[i]);
+      q[a] = fmaf(pr, pr, q[a]);
+      const float pm = V::round_prod(pr);
+      if (pm < mn[a]) { mn[a] = pm; amn[a] = jabs; }
+      if (pm > mx[a]) { mx[a] = pm; amx[a] = jabs; }
+    }
+  }
+
+  // ring-relative nnz [s, e) of one row, G entries per step (one per lane group) and U steps per chunk, as
+  // RowEngine::accumulate walks them
+  __device__ __forceinline__ void accumulate(IndexRing<T>& ring, int s0, int e, const char* __restrict__ matb,
+                                             uint32_t row_bytes, const bool (&col_ok)[CH], int lane, int g,
+                                             uint64_t pol) {
+    using VR = typename V::vraw;
+    for (int j0 = s0; j0 < e; j0 += U * G) {
+      const int jend = min(e, j0 + U * G);
+      ring.ensure(j0, jend, lane);
+      const int slot0 = (j0 + g) & (kRing - 1);
+      const uint32_t* pc = reinterpret_cast<const uint32_t*>(ring.s_col + slot0);
+      const VR* pv = reinterpret_cast<const VR*>(ring.s_val) + slot0;
+      const int jabs0 = (int)ring.base + j0 + g;
+      const int nst = (jend - j0 + G - 1) / G;
+      const int jrel = jend - j0 - g;
+      uint4 d[U][CH];
+      VR v[U];
+      bool act[U];
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        if (u >= nst) break;
+        act[u] = u * G < jrel;
+        const uint32_t c = pc[2 * u * G];
+        v[u] = pv[u * G];
+        const char* src = matb + (uint64_t)c * row_bytes;
+#pragma unroll
+        for (int ch = 0; ch < CH; ch++)
+          if (act[u] && col_ok[ch]) d[u][ch] = ldg128_hint(src + ch * (LPR * 16), pol);
+      }
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        if (u >= nst) break;
+#pragma unroll
+        for (int ch = 0; ch < CH; ch++)
+          if (act[u] && col_ok[ch]) step(ch, v[u], d[u][ch], jabs0 + u * G);
+      }
+    }
+  }
+
+  // the butterfly of RowEngine::reduce_groups over the four statistics
+  __device__ __forceinline__ void reduce_groups() {
+#pragma unroll
+    for (int off = LPR; off < 32; off <<= 1) {
+#pragma unroll
+      for (int i = 0; i < NA; i++) {
+        s[i] += __shfl_xor_sync(0xffffffffu, s[i], off);
+        q[i] += __shfl_xor_sync(0xffffffffu, q[i], off);
+        const float on = __shfl_xor_sync(0xffffffffu, mn[i], off);
+        const int oan = __shfl_xor_sync(0xffffffffu, amn[i], off);
+        if (on < mn[i] || (on == mn[i] && oan < amn[i])) { mn[i] = on; amn[i] = oan; }
+        const float ox = __shfl_xor_sync(0xffffffffu, mx[i], off);
+        const int oax = __shfl_xor_sync(0xffffffffu, amx[i], off);
+        if (ox > mx[i] || (ox == mx[i] && oax < amx[i])) { mx[i] = ox; amx[i] = oax; }
+      }
+    }
+  }
+
+  // final write of row `row` (count entries) by the lanes that hold it: each requested aggregator into its slice, the
+  // args where their pointers are set
+  __device__ __forceinline__ void store_row(const SpmmParams& p, const MultiOut& mo, int64_t row, int64_t count,
+                                            const bool (&col_ok)[CH], int li) const {
+    T* orow = (T*)p.out + row * mo.A * p.K + p.k0;
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) {
+      if (!col_ok[ch]) continue;
+      const int koff = (ch * LPR + li) * VEC;
+#pragma unroll
+      for (int c = 0; c < kStats; c++) {
+        const int sl = mo.slice[c];
+        if (sl < 0) continue;
+        float f[VEC];
+#pragma unroll
+        for (int i = 0; i < VEC; i++) {
+          const int a = ch * VEC + i;
+          f[i] = multi_stat<float>(c, s[a], q[a], mn[a], mx[a], count);
+        }
+        stg128_stream(orow + sl * p.K + koff, V::pack(f));
+      }
+      if (mo.arg_min) store_args<VEC>(mo.arg_min + row * p.K + p.k0 + koff, &amn[ch * VEC], count, p.E);
+      if (mo.arg_max) store_args<VEC>(mo.arg_max + row * p.K + p.k0 + koff, &amx[ch * VEC], count, p.E);
+    }
+  }
+
+  // the partial of one segment into slot `slot`: four fp32 planes [slot][4][K] (S, Q, min, max) and two int64 arg
+  // planes [slot][2][K] (min, max)
+  __device__ __forceinline__ void store_partial(const SpmmParams& p, int64_t slot, const bool (&col_ok)[CH],
+                                                int li) const {
+    float* pv = (float*)p.part_val + slot * 4 * p.K + p.k0;
+    int64_t* pa = p.part_arg + slot * 2 * p.K + p.k0;
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) {
+      if (!col_ok[ch]) continue;
+      const int koff = (ch * LPR + li) * VEC;
+#pragma unroll
+      for (int i = 0; i < VEC; i++) {
+        const int a = ch * VEC + i;
+        pv[koff + i] = s[a];
+        pv[p.K + koff + i] = q[a];
+        pv[2 * p.K + koff + i] = mn[a];
+        pv[3 * p.K + koff + i] = mx[a];
+        pa[koff + i] = stored_arg(amn[a], p.E);
+        pa[p.K + koff + i] = stored_arg(amx[a], p.E);
+      }
+    }
+  }
+};
+
+// column kk of a multi-segment row: its partials folded in segment order as combine_col folds them (the smallest e
+// wins min / max ties), then every requested aggregator and arg stored. CG: read past L1 (planned drain).
+template <typename T, bool CG>
+__device__ __forceinline__ void combine_multi_col(const SpmmParams& p, const MultiOut& mo, const LongRow& L, int nseg,
+                                                  int64_t count, int64_t kk) {
+  const float* pv = (const float*)p.part_val;
+  auto ldv = [&](int64_t sl, int st) {
+    const float* a = pv + (sl * 4 + st) * p.K + kk;
+    return CG ? __ldcg(a) : *a;
+  };
+  auto lda = [&](int64_t sl, int st) {
+    const int64_t* a = p.part_arg + (sl * 2 + st) * p.K + kk;
+    return CG ? __ldcg(a) : *a;
+  };
+  float s = ldv(L.first_slot, 0), q = ldv(L.first_slot, 1), mn = ldv(L.first_slot, 2), mx = ldv(L.first_slot, 3);
+  int64_t amn = lda(L.first_slot, 0), amx = lda(L.first_slot, 1);
+  for (int sgi = 1; sgi < nseg; sgi++) {
+    const int64_t sl = L.first_slot + sgi;
+    s += ldv(sl, 0);
+    q += ldv(sl, 1);
+    const float vn = ldv(sl, 2), vx = ldv(sl, 3);
+    const int64_t an = lda(sl, 0), ax = lda(sl, 1);
+    if (vn < mn || (vn == mn && an < amn)) { mn = vn; amn = an; }
+    if (vx > mx || (vx == mx && ax < amx)) { mx = vx; amx = ax; }
+  }
+  T* orow = (T*)p.out + L.row_b * mo.A * p.K + kk;
+#pragma unroll
+  for (int c = 0; c < kStats; c++)
+    if (mo.slice[c] >= 0) orow[mo.slice[c] * p.K] = Traits<T>::from_acc(multi_stat<float>(c, s, q, mn, mx, count));
+  if (mo.arg_min) mo.arg_min[L.row_b * p.K + kk] = amn;
+  if (mo.arg_max) mo.arg_max[L.row_b * p.K + kk] = amx;
+}
+
+__device__ __forceinline__ void long_row_counts(const LongRow& L, int& nseg, int64_t& count) {
+  nseg = (int)(L.nseg_count >> 40);
+  count = L.nseg_count & (((int64_t)1 << 40) - 1);
+}
+
+// row-per-warp multi kernel: the work items of spmm_vec_kernel and, PLAN with DRAIN, its drain of the plan's segments
+template <typename T, int LPR, int CH, int U, int MINB, bool PLAN, bool DRAIN>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
+spmm_multi_vec_kernel(const SpmmParams p, const MultiOut mo) {
+  using Eng = MultiEngine<T, LPR, CH, U>;
+  constexpr int VEC = Eng::VEC;
+  __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
+  __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane / LPR, li = lane % LPR;
+
+  IndexRing<T> ring;
+  ring.template bind<true>(p, s_col[warp], s_val[warp], lane);
+  const uint64_t pol = make_policy_evict_last();
+  bool col_ok[CH];
+  int hcol[1];
+  uint32_t row_bytes;
+  int64_t lane_off;
+  lane_cols<T, LPR, VEC, CH, false>(p, li, col_ok, hcol, row_bytes, lane_off);
+
+  for (WorkItem it(p, lane); it.start(p, lane); it.advance()) {
+    const int64_t a0 = __shfl_sync(0xffffffffu, it.rp0, 0);
+    const int64_t base = a0 & ~(int64_t)31;
+    const int s_rel = (int)(it.rp0 - base), e_rel = (int)(it.rp1 - base);
+    const int deg = e_rel - s_rel;
+    unsigned defer_mask;
+    if constexpr (PLAN) {
+      defer_mask = it.plan_defer_mask(p);
+    } else {
+      const bool defer = defer_row(deg, lane);
+      defer_mask = __ballot_sync(0xffffffffu, defer);
+      if (defer) push_row_segments(p, it.b, it.r0, lane, it.rp0, it.rp1, deg);
+    }
+    __syncwarp();
+    ring.reset(base, __shfl_sync(0xffffffffu, it.rp1, 31));
+    const char* matb = (const char*)p.mat + lane_off;
+    asm volatile("" : "+l"(matb));
+    for (int rl = 0; rl < it.nrows; rl++) {
+      if ((defer_mask >> rl) & 1u) continue;
+      const int s = __shfl_sync(0xffffffffu, s_rel, rl);
+      const int e = __shfl_sync(0xffffffffu, e_rel, rl);
+      Eng eng;
+      eng.init();
+      eng.accumulate(ring, s, e, matb, row_bytes, col_ok, lane, g, pol);
+      eng.reduce_groups();
+      if (g == 0) eng.store_row(p, mo, it.r0 + rl, e - s, col_ok, li);
+    }
+  }
+
+  if constexpr (PLAN && DRAIN) {  // the planned drain of spmm_vec_kernel
+    constexpr int kcols = LPR * CH * VEC;
+    while (true) {
+      const unsigned int sidx = __shfl_sync(0xffffffffu, take_ticket(&p.counters[5], lane), 0);
+      if ((int64_t)sidx >= p.n_seg) break;
+      const Segment S = p.segs[sidx];
+      Eng eng;
+      walk_segment<false>(eng, p, S, 0, ring, col_ok, hcol, row_bytes, lane_off, lane, g, pol);
+      if (S.slot < 0) {
+        if (g == 0) eng.store_row(p, mo, S.row_b, S.end - S.start, col_ok, li);
+      } else {
+        if (g == 0) eng.store_partial(p, S.slot, col_ok, li);
+        __syncwarp();
+        __threadfence();
+        const uint32_t lr = __ldg(p.seg_lr + sidx);
+        unsigned int finished = 0;
+        if (lane == 0) finished = atomicAdd(&p.long_done[lr], 1u);
+        finished = __shfl_sync(0xffffffffu, finished, 0);
+        const LongRow L = p.longs[lr];
+        int nseg;
+        int64_t count;
+        long_row_counts(L, nseg, count);
+        if ((int)finished == nseg - 1) {
+          __threadfence();
+          for (int k = lane; k < kcols && p.k0 + k < p.K; k += 32)
+            combine_multi_col<T, true>(p, mo, L, nseg, count, p.k0 + k);
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// group-per-row multi kernel (narrow rows): the walk of spmm_gpr_kernel, each lane group over its own row
+template <typename T, int LPR, int U, int MINB, bool PLAN>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
+spmm_multi_gpr_kernel(const SpmmParams p, const MultiOut mo) {
+  using V = Vec<T>;
+  using Eng = MultiEngine<T, LPR, 1, U>;
+  using VR = typename V::vraw;
+  constexpr int VEC = Eng::VEC;
+  constexpr int G = 32 / LPR;
+  const int lane = threadIdx.x & 31;
+  const int g = lane / LPR, li = lane % LPR;
+  const bool col_ok = p.k0 + li * VEC < p.K;
+  const uint32_t row_bytes = (uint32_t)(p.K * (int64_t)sizeof(T));
+  const int64_t lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(T);
+  const uint64_t pol = make_policy_evict_last();
+  const T* __restrict__ val = (const T*)p.value;
+  const bool has_val = val != nullptr;
+
+  for (WorkItem it(p, lane); it.start(p, lane); it.advance()) {
+    const int64_t base = __shfl_sync(0xffffffffu, it.rp0, 0);
+    const int s_rel = (int)(it.rp0 - base), e_rel = (int)(it.rp1 - base);
+    const int deg = e_rel - s_rel;
+    unsigned defer_mask;
+    if constexpr (PLAN) {
+      defer_mask = it.plan_defer_mask(p);
+    } else {
+      const bool defer = defer_row(deg, lane);
+      defer_mask = __ballot_sync(0xffffffffu, defer);
+      if (defer) push_row_segments(p, it.b, it.r0, lane, it.rp0, it.rp1, deg);
+    }
+    __syncwarp();
+    const char* matb = (const char*)p.mat + lane_off;
+    asm volatile("" : "+l"(matb));
+    const int64_t* __restrict__ colb = p.col + base;
+    const T* __restrict__ valb = has_val ? val + base : nullptr;
+    const bool col_ok_arr[1] = {col_ok};
+    const int jbase = (int)base;
+
+    for (int t = 0; t < it.nrows; t += G) {
+      const int rl = t + g;
+      int s = __shfl_sync(0xffffffffu, s_rel, rl & 31);
+      int e = __shfl_sync(0xffffffffu, e_rel, rl & 31);
+      const bool mine = rl < it.nrows && !((defer_mask >> (rl & 31)) & 1u);
+      if (!mine) e = s;
+      const int len = e - s;
+      int maxlen = len;
+#pragma unroll
+      for (int off = LPR; off < 32; off <<= 1) maxlen = max(maxlen, __shfl_xor_sync(0xffffffffu, maxlen, off));
+      Eng eng;
+      eng.init();
+      uint32_t cn[U];
+      VR vn[U];
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        cn[u] = 0;
+        vn[u] = V::one();
+        if (u < len) {
+          cn[u] = (uint32_t)__ldg(colb + s + u);
+          if (has_val) vn[u] = load_vraw<T>(valb + s + u);
+        }
+      }
+      for (int j0 = 0; j0 < maxlen; j0 += U) {
+        uint4 d[U];
+        VR v[U];
+        bool act[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+          act[u] = (j0 + u < len) && col_ok;
+          v[u] = vn[u];
+          if (act[u]) d[u] = ldg128_hint(matb + (uint64_t)cn[u] * row_bytes, pol);
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+          const int jn = j0 + U + u;
+          if (jn < len) {
+            cn[u] = (uint32_t)__ldg(colb + s + jn);
+            if (has_val) vn[u] = load_vraw<T>(valb + s + jn);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++)
+          if (act[u]) eng.step(0, v[u], d[u], jbase + s + j0 + u);
+      }
+      if (mine) eng.store_row(p, mo, it.r0 + rl, len, col_ok_arr, li);
+    }
+  }
+}
+
+// one warp per queued segment (spmm_seg_kernel)
+template <typename T, int LPR, int CH, int U, int MINB>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, MINB)
+spmm_multi_seg_kernel(const SpmmParams p, const MultiOut mo) {
+  using Eng = MultiEngine<T, LPR, CH, U>;
+  constexpr int VEC = Eng::VEC;
+  __shared__ __align__(16) int64_t s_col[kWarpsPerCta][kRingAlloc];
+  __shared__ __align__(16) T s_val[kWarpsPerCta][kRingAlloc];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane / LPR, li = lane % LPR;
+  IndexRing<T> ring;
+  ring.template bind<true>(p, s_col[warp], s_val[warp], lane);
+  const uint64_t pol = make_policy_evict_last();
+  bool col_ok[CH];
+  int hcol[1];
+  uint32_t row_bytes;
+  int64_t lane_off;
+  lane_cols<T, LPR, VEC, CH, false>(p, li, col_ok, hcol, row_bytes, lane_off);
+
+  const int64_t nseg = p.plan_mask ? p.n_seg : min((int64_t)p.counters[1], p.seg_cap);
+  const int64_t wstride = (int64_t)gridDim.x * kWarpsPerCta;
+  for (int64_t sidx = (int64_t)blockIdx.x * kWarpsPerCta + warp; sidx < nseg; sidx += wstride) {
+    const Segment S = p.segs[sidx];
+    Eng eng;
+    walk_segment<false>(eng, p, S, 0, ring, col_ok, hcol, row_bytes, lane_off, lane, g, pol);
+    if (g == 0) {
+      if (S.slot < 0) eng.store_row(p, mo, S.row_b, S.end - S.start, col_ok, li);
+      else eng.store_partial(p, S.slot, col_ok, li);
+    }
+    __syncwarp();
+  }
+}
+
+// the multi-segment rows' partials, in segment order (spmm_combine_kernel)
+template <typename T>
+__global__ void spmm_multi_combine_kernel(const SpmmParams p, const MultiOut mo, int kcols) {
+  const int64_t nlong = p.plan_mask ? p.n_long : min((int64_t)p.counters[2], p.long_cap);
+  for (int64_t li = blockIdx.x; li < nlong; li += gridDim.x) {
+    const LongRow L = p.longs[li];
+    int nseg;
+    int64_t count;
+    long_row_counts(L, nseg, count);
+    for (int k = threadIdx.x; k < kcols && p.k0 + k < p.K; k += blockDim.x)
+      combine_multi_col<T, false>(p, mo, L, nseg, count, p.k0 + k);
+  }
+}
+
+// generic multi kernel (fp64, partial widths, unaligned operands, E >= 2^31): warp per row, lane per column, the entries
+// in order as spmm_generic_kernel walks them (one rounding per product and per sum), plus Q = sum fma(p, p, .)
+template <typename T>
+__global__ void __launch_bounds__(256)
+spmm_multi_generic_kernel(const int64_t* __restrict__ rowptr, const int64_t* __restrict__ col,
+                          const T* __restrict__ value, const T* __restrict__ mat, T* __restrict__ out, int64_t M,
+                          int64_t K, int64_t E, const MultiOut mo) {
+  using acc_t = typename Traits<T>::acc_t;
+  constexpr bool F64 = std::is_same<acc_t, double>::value;
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t m = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; m < M; m += nw) {
+    const int64_t rs = rowptr[m], re = rowptr[m + 1];
+    for (int64_t k = lane; k < K; k += 32) {
+      acc_t s = 0, q = 0;
+      acc_t mn = Traits<T>::to_acc(Traits<T>::highest()), mx = Traits<T>::to_acc(Traits<T>::lowest());
+      int64_t amn = E, amx = E;
+      for (int64_t e = rs; e < re; e++) {
+        const acc_t mv = Traits<T>::to_acc(mat[col[e] * K + k]);
+        acc_t pr = mv;
+        if (value) {
+          if constexpr (F64) pr = __dmul_rn(Traits<T>::to_acc(value[e]), mv);
+          else pr = __fmul_rn(Traits<T>::to_acc(value[e]), mv);
+        }
+        if constexpr (F64) { s = __dadd_rn(s, pr); q = fma(pr, pr, q); }
+        else { s = __fadd_rn(s, pr); q = fmaf(pr, pr, q); }
+        acc_t pm = pr;
+        if constexpr (is_float16<T>::value) pm = Traits<T>::to_acc(Traits<T>::from_acc(pr));
+        if (pm < mn) { mn = pm; amn = e; }
+        if (pm > mx) { mx = pm; amx = e; }
+      }
+      const int64_t cnt = re - rs;
+#pragma unroll
+      for (int c = 0; c < kStats; c++)
+        if (mo.slice[c] >= 0)
+          out[(m * mo.A + mo.slice[c]) * K + k] = Traits<T>::from_acc(multi_stat<acc_t>(c, s, q, mn, mx, cnt));
+      if (mo.arg_min) mo.arg_min[m * K + k] = cnt > 0 ? amn : E;
+      if (mo.arg_max) mo.arg_max[m * K + k] = cnt > 0 ? amx : E;
+    }
+  }
+}
+
+// workspace of tsb200_spmm_fw_multi: the layouts of tsb200_spmm_fw (plan == NULL) or tsb200_spmm_fw_planned over 4 * K
+// fp32 partial columns per slot, followed by 2 * K int64 arg columns per slot
+struct MultiWs {
+  size_t args, total;
+};
+static inline MultiWs multi_ws(int64_t K, int64_t E, bool planned, int64_t n_long, int64_t n_slot) {
+  MultiWs L;
+  const int64_t slots = planned ? (n_slot > 0 ? n_slot : 1) : ws_layout(1, K, E, false).slot_cap;
+  L.args = planned ? planned_ws(4 * K, n_long, n_slot, false).total : ws_layout(1, 4 * K, E, false).total;
+  L.total = L.args + align_up((size_t)slots * (size_t)(2 * K) * sizeof(int64_t), 256);
+  return L;
+}
+
+template <typename T, int LPR, int CH, int U, int MINB, bool GPR, bool PLAN>
+static int launch_multi(SpmmParams p, const MultiOut& mo, cudaStream_t st) {
+  constexpr int kcols = LPR * CH * Vec<T>::VEC;
+  // the planned drain spills the 16-bit kernel of the widest shape (four statistics of 32 columns per lane), so there
+  // the plan's segments go to the segment and combine kernels, as for the group-per-row shapes
+  constexpr bool DRAIN = !GPR && !(sizeof(T) == 2 && CH == 4);
+  void (*kmain)(const SpmmParams, const MultiOut);
+  if constexpr (GPR) kmain = spmm_multi_gpr_kernel<T, LPR, U, MINB, PLAN>;
+  else kmain = spmm_multi_vec_kernel<T, LPR, CH, U, MINB, PLAN, DRAIN>;
+  constexpr int USEG = (U > LPR) ? LPR : U;
+  auto* kseg = spmm_multi_seg_kernel<T, LPR, CH, USEG, MINB>;
+  static GridCache gc_main, gc_seg;
+  for (int k0 = 0; k0 < p.K; k0 += kcols) {
+    p.k0 = k0;
+    if constexpr (PLAN) {  // as launch_vec: one kernel, plus segment / combine kernels when it does not drain
+      const int grid_main = gc_main.get((const void*)kmain, kWarpsPerCta * 32);
+      p.item_shift = item_shift_for(p.M, grid_main);
+      const int64_t n_items = (p.M + (1 << p.item_shift) - 1) >> p.item_shift;
+      TSB_CUDA_TRY(cudaMemsetAsync(p.counters, 0, 256 + (size_t)p.n_long * 4, st));
+      int64_t work = (n_items + kWarpsPerCta - 1) / kWarpsPerCta;
+      if (DRAIN) work = max(work, (p.n_seg + kWarpsPerCta - 1) / kWarpsPerCta);
+      kmain<<<(int)max((int64_t)1, min((int64_t)grid_main, work)), kWarpsPerCta * 32, 0, st>>>(p, mo);
+      TSB_LAUNCH_CHECK();
+      if (!DRAIN && p.n_seg > 0) {
+        kseg<<<gc_seg.get((const void*)kseg, kWarpsPerCta * 32), kWarpsPerCta * 32, 0, st>>>(p, mo);
+        TSB_LAUNCH_CHECK();
+        if (p.n_long > 0) {
+          spmm_multi_combine_kernel<T><<<num_sms() * 2, 128, 0, st>>>(p, mo, kcols);
+          TSB_LAUNCH_CHECK();
+        }
+      }
+    } else {
+      if (const int rc = launch_rowsplit(kmain, kseg, gc_main, gc_seg, p, st, mo)) return rc;
+      spmm_multi_combine_kernel<T><<<num_sms() * 2, 128, 0, st>>>(p, mo, kcols);
+      TSB_LAUNCH_CHECK();
+    }
+  }
+  return 0;
+}
+
+// (LPR, CH) of dispatch_shape for each row width, so that every lane sums, compares and folds as the single-reduction
+// kernels do; (U, CTAs/SM) the most CTAs/SM at which ptxas reports no spill for the four statistics (DESIGN §3.1)
+// (the 16-bit wide shapes hold twice the columns per lane of fp32 ones, so they take fewer CTAs and gathers in flight)
+template <typename T, bool PLAN>
+static int dispatch_multi(const SpmmParams& p, const MultiOut& mo, cudaStream_t st) {
+  constexpr bool W16 = sizeof(T) == 2;
+  const int64_t vecs = p.K / Vec<T>::VEC;
+  if (vecs <= 1) return launch_multi<T, 1, 1, 4, 2, true, PLAN>(p, mo, st);
+  if (vecs <= 2) return launch_multi<T, 2, 1, 4, 2, true, PLAN>(p, mo, st);
+  if (vecs <= 4) return launch_multi<T, 4, 1, 4, 2, true, PLAN>(p, mo, st);
+  if (vecs <= 8) return launch_multi<T, 8, 1, 4, 2, true, PLAN>(p, mo, st);
+  if (vecs <= 16) return launch_multi<T, 16, 1, 4, 2, false, PLAN>(p, mo, st);
+  if (vecs <= 32) return launch_multi<T, 32, 1, 4, 2, false, PLAN>(p, mo, st);
+  if (vecs <= 64) return launch_multi<T, 32, 2, 2, W16 ? 1 : 2, false, PLAN>(p, mo, st);
+  return launch_multi<T, 32, 4, W16 ? 1 : 2, 1, false, PLAN>(p, mo, st);
+}
+
 }  // namespace tsb
 
 using namespace tsb;
@@ -1813,3 +2361,59 @@ extern "C" int tsb200_spmm_heads(const int64_t* rowptr, const int64_t* col, cons
     return 0;
   });
 }
+
+// ---- multi-aggregation SpMM (tsb200_spmm_fw_multi) ------------------------------------------------------------------
+// The definitions take their C linkage from the declarations in tsb200.h (see tsb200_spmm_fw_res and the guards below).
+size_t tsb200_spmm_fw_multi_workspace_bytes(int64_t K, int64_t E, int planned, int64_t n_long, int64_t n_slot) {
+  if (K <= 0 || E <= 0 || n_long < 0 || n_slot < 0) return 0;
+  return multi_ws(K, E, planned != 0, n_long, n_slot).total;
+}
+
+int tsb200_spmm_fw_multi(const int64_t* rowptr, const int64_t* col, const void* value, const void* mat,
+                         const int* aggrs, int n_aggr, void* out, int64_t* arg_min, int64_t* arg_max, int64_t M,
+                         int64_t N, int64_t K, int64_t E, int dtype, const void* plan, size_t plan_bytes, int64_t n_seg,
+                         int64_t n_long, int64_t n_slot, void* workspace, size_t workspace_bytes, void* stream) {
+  if (M < 0 || N < 0 || K < 0 || E < 0 || n_seg < 0 || n_long < 0 || n_slot < 0) return TSB200_ERR_INVALID_ARG;
+  if (!aggrs || n_aggr < 1 || n_aggr > kStats) return TSB200_ERR_INVALID_ARG;
+  MultiOut mo{arg_min, arg_max, n_aggr, {-1, -1, -1, -1, -1, -1}};
+  for (int a = 0; a < n_aggr; a++) {
+    const int c = aggrs[a];
+    if (c < TSB200_SUM || c > TSB200_STD || mo.slice[c] >= 0) return TSB200_ERR_INVALID_ARG;
+    mo.slice[c] = (int8_t)a;
+  }
+  if ((arg_min && mo.slice[R_MIN] < 0) || (arg_max && mo.slice[R_MAX] < 0)) return TSB200_ERR_INVALID_ARG;
+  if (dtype_size(dtype) == 0) return TSB200_ERR_INVALID_ARG;
+  if (dtype != TSB200_F32 && dtype != TSB200_F64 && dtype != TSB200_F16 && dtype != TSB200_BF16)
+    return TSB200_ERR_UNSUPPORTED;
+  if (M * K == 0) return 0;  // nothing to write
+  if (!rowptr || !out) return TSB200_ERR_INVALID_ARG;
+  if (E > 0 && (!col || !mat)) return TSB200_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+
+  if (E > 0 && vec_eligible(dtype, K, E, N, value, mat, out, col, arg_min) && !((uintptr_t)arg_max & 15)) {
+    SpmmParams p{rowptr, col, value, mat, out, nullptr, 1, M, N, K, E};
+    // the fp32 planes bound as a workspace of 4 * K partial columns, the arg planes behind them
+    const MultiWs L = multi_ws(K, E, plan != nullptr, n_long, n_slot);
+    SpmmParams q = p;
+    q.K = 4 * K;
+    if (const int rc = bind_workspace(q, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, false))
+      return rc;
+    if (workspace_bytes < L.total) return TSB200_ERR_WORKSPACE;
+    q.K = K;
+    q.part_arg = (int64_t*)((char*)workspace + L.args);
+    return dispatch_vec_dtype(dtype, [&](auto tag) {
+      using T = decltype(tag);
+      return plan ? dispatch_multi<T, true>(q, mo, st) : dispatch_multi<T, false>(q, mo, st);
+    });
+  }
+  return dispatch_float_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    spmm_multi_generic_kernel<T><<<warp_grid(M, 64), 256, 0, st>>>(rowptr, col, (const T*)value, (const T*)mat,
+                                                                   (T*)out, M, K, E, mo);
+    TSB_LAUNCH_CHECK();
+    return 0;
+  });
+}
+[[maybe_unused]] static constexpr auto tsb200_spmm_fw_multi_declared_once = &tsb200_spmm_fw_multi;
+[[maybe_unused]] static constexpr auto tsb200_spmm_fw_multi_workspace_bytes_declared_once =
+    &tsb200_spmm_fw_multi_workspace_bytes;

@@ -6,7 +6,7 @@ reference's these functions are TorchScript-compatible (`torch.jit.script(spspmm
 native step is a registered operator. A reduction materialises only the cached CSR/CSC views a requested gradient
 will read (the reference's rule, :19-25, :46-53).
 """
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -110,6 +110,35 @@ def spmm(src: SparseTensor, other: Tensor, reduce: str = "sum", residual: Option
         return spmm_max(src, other)[0]
     else:
         raise ValueError("unknown reduce '" + reduce + "'")
+
+
+def spmm_multi(src: SparseTensor, other: Tensor, aggrs: List[str]) -> Tensor:
+    """Several aggregations of every row's messages value[e] * other[col[e]] from one gather pass: out [M, A, K] holds
+    aggregator aggrs[a] in out[:, a] (sum / add, mean, min, max, var, std; each at most once), and `out.flatten(1)` is
+    their feature-dim concatenation, as PNA and multi-aggregation layers use it. sum, mean, min and max are bit for bit
+    `spmm`'s. With n = max(degree, 1): var = max(Q / n - mean^2, 0), Q the fp32 (fp64) sum of squared messages, and
+    std = sqrt(var) where var > 1e-5, else 0; neither passes a gradient where its clamp is active, which keeps the
+    gradient finite on constant and one-entry rows. `other` is 2-D (bf16, f16, f32, f64). Differentiable in the values
+    and `other`; only the caches a requested gradient reads are built."""
+    if other.dim() != 2:
+        raise RuntimeError("spmm_multi: other must be 2-D [N, K], got " + str(other.dim()) + "-D")
+    N = src.size(1)
+    if other.size(0) != N:
+        raise RuntimeError("spmm_multi: other must have " + str(N) + " rows (the sparse sizes), got " + str(other.size(0)))
+    rowptr, col, value = src.csr()
+    st = src.storage
+    row, colptr, csr2csc = st._row, st._colptr, st._csr2csc
+    row_csc: Optional[Tensor] = None
+    if value is not None:
+        value = value.to(other.dtype)
+        if value.requires_grad:
+            row = st.row()
+    if other.requires_grad:     # A^T a and A_{v^2}^T b run on the CSC view
+        row = st.row()
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.spmm_multi(row, rowptr, col, value, colptr, csr2csc, other, row_csc, aggrs)
 
 
 def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
@@ -318,6 +347,7 @@ SparseTensor.sddmm = lambda self, a, b: sddmm(self, a, b)
 SparseTensor.sddmm_fp8 = lambda self, a8, a_scale, b8, b_scale, out_dtype=torch.float32: sddmm_fp8(
     self, a8, a_scale, b8, b_scale, out_dtype)
 SparseTensor.spmm_heads = lambda self, x: spmm_heads(self, x)
+SparseTensor.spmm_multi = lambda self, other, aggrs: spmm_multi(self, other, aggrs)
 SparseTensor.sddmm_heads = lambda self, a, b: sddmm_heads(self, a, b)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)

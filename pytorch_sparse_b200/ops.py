@@ -11,7 +11,7 @@ from __future__ import annotations
 import collections
 import ctypes
 import os
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -303,6 +303,83 @@ def spmm_fw_res(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tenso
                                      _p(out), M, N, K, E, dt, red, *pl, _p(ws), nws, _stream(dev)),
               "tsb200_spmm_fw_res")
     return out
+
+
+# aggregator codes of tsb200_spmm_fw_multi: the reduce codes plus TSB200_VAR / TSB200_STD
+_AGGR = {"sum": 0, "add": 0, "mean": 1, "min": 2, "max": 3, "var": 4, "std": 5}
+
+
+def _aggr_codes(aggrs: List[str]) -> List[int]:
+    if len(aggrs) == 0:
+        raise ValueError("spmm_multi: aggrs must name at least one aggregator")
+    codes: List[int] = []
+    for a in aggrs:
+        c = _AGGR.get(a)
+        if c is None:
+            raise ValueError(f"spmm_multi: unknown aggregator '{a}' (expected sum, add, mean, min, max, var or std)")
+        if c in codes:
+            raise ValueError(f"spmm_multi: aggregator '{a}' is given more than once")
+        codes.append(c)
+    return codes
+
+
+def _spmm_fw_multi(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, codes: List[int],
+                   want_args: bool, plan: Optional[SpmmPlan] = None):
+    _check_cuda(rowptr, "rowptr")
+    _check_cuda(col, "col")
+    if value is not None:
+        _check_cuda(value, "optional_value.value()")
+    _check_cuda(mat, "mat")
+    if mat.dim() != 2:
+        raise RuntimeError(f"spmm_multi: the dense operand must be 2-D [N, K], got {mat.dim()}-D")
+    _check_input(rowptr.dim() == 1)
+    _check_input(col.dim() == 1)
+    if value is not None:
+        _check_input(value.dim() == 1)
+        _check_input(value.size(0) == col.size(0))
+        if value.dtype != mat.dtype:
+            raise RuntimeError(f"expected value of dtype {mat.dtype} but got {value.dtype}")
+        value = value.contiguous()
+    rowptr = _i64(rowptr, "rowptr")
+    col = _i64(col, "col")
+    mat = mat.contiguous()
+    dt = _dtype_code(mat.dtype)
+    M = rowptr.numel() - 1
+    N, K = mat.shape
+    E = col.numel()
+    dev = mat.device
+    out = torch.empty(M, len(codes), K, dtype=mat.dtype, device=dev)
+    arg_min = torch.empty(M, K, dtype=torch.int64, device=dev) if want_args and 2 in codes else None
+    arg_max = torch.empty(M, K, dtype=torch.int64, device=dev) if want_args and 3 in codes else None
+    if out.numel() == 0:
+        return out, arg_min, arg_max
+    with _on_device(dev):
+        plannable = E > 0 and dt in (0, 2, 3) and (K * mat.element_size()) % 16 == 0
+        if plannable and plan is None:
+            plan = _auto_plan(rowptr, E)
+        if plannable and plan is not None and plan.M == M and plan.E == E:
+            nws = lib.tsb200_spmm_fw_multi_workspace_bytes(K, E, 1, plan.n_long, plan.n_slot)
+            pl = (_p(plan.data), plan.data.numel(), plan.n_seg, plan.n_long, plan.n_slot)
+        else:
+            nws = lib.tsb200_spmm_fw_multi_workspace_bytes(K, E, 0, 0, 0)
+            pl = (None, 0, 0, 0, 0)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_fw_multi(_p(rowptr), _p(col), _p(value), _p(mat), (ctypes.c_int * len(codes))(*codes),
+                                       len(codes), _p(out), _p(arg_min), _p(arg_max), M, N, K, E, dt, *pl, _p(ws), nws,
+                                       _stream(dev)), "tsb200_spmm_fw_multi")
+    return out, arg_min, arg_max
+
+
+def spmm_fw_multi(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, aggrs: List[str],
+                  want_args: bool = False,
+                  plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor], Optional[Tensor]]:
+    """`out [M, A, K]`: aggregator aggrs[a] (sum / add, mean, min, max, var, std) of every row's messages
+    value[e] * mat[col[e]] in out[:, a], from one gather pass (tsb200_spmm_fw_multi). The sum, mean, min and max
+    slices are bit for bit `spmm_fw`'s on the same path. var = max(Q / n - mean^2, 0) with Q the fp32 (fp64) sum of
+    squared messages and n = max(degree, 1); std = sqrt(var) where var > 1e-5, else 0. `mat` is 2-D [N, K] (bf16,
+    f16, f32, f64). want_args: also return arg_min / arg_max [M, K] (None for an aggregator not requested), as
+    `spmm_fw` returns arg_out. Planned like `spmm_fw` (the same per-rowptr plan cache). Forward only: see SPMMMulti."""
+    return _spmm_fw_multi(rowptr, col, value, mat, _aggr_codes(aggrs), want_args, plan)
 
 
 _FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
@@ -1210,6 +1287,112 @@ class SPMMRes(torch.autograd.Function):
             gr = grad_out.to(acc) * residual.to(acc)
             grad_scale = gr.sum(1) if scale.dim() == 1 else gr.sum()
         return (None, None, None, grad_value, None, None, None, grad_mat, None, grad_res, grad_scale, None)
+
+
+class SPMMMulti(torch.autograd.Function):
+    """`spmm_fw_multi`, differentiable in the values and `mat` with no kernel of its own. With g_c the gradient of
+    slice c, n = max(degree, 1), mu the mean and g_v = g_var [var > 0] + g_std / (2 std) [std > 0] (the clamps of var
+    and std pass no gradient), per row a = g_sum + g_mean / n - 2 mu g_v / n and b = 2 g_v / n, so that the gradient of
+    every message p_e = v_e x[col_e] is a + b p_e:
+        grad_x = A^T a + x * (A_{v^2}^T b)          (two SpMMs on the CSC view; A_{v^2} has the values v^2)
+        grad_v[e] = <a_row, x_col> + v_e <b_row, x_col^2>   (two SDDMMs)
+    plus the min / max gradients of spmm_minmax_bw. Terms without a gradient are skipped. The mean is computed as an
+    extra slice when var / std need a gradient and it is not requested."""
+    @staticmethod
+    def forward(ctx, row, rowptr, col, value, colptr, csr2csc, mat, row_csc, aggrs):
+        codes = _aggr_codes(aggrs)
+        need_value = value is not None and ctx.needs_input_grad[3]
+        need_mat = ctx.needs_input_grad[6]
+        if need_value or need_mat:
+            _assert_present(row, "row")
+        if need_mat:
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+        need = need_value or need_mat
+        kcodes = list(codes)
+        if need and (4 in codes or 5 in codes) and 1 not in codes:
+            kcodes.append(1)
+        full, arg_min, arg_max = _spmm_fw_multi(rowptr, col, value, mat, kcodes, need)
+        out = full if len(kcodes) == len(codes) else full[:, :len(codes)].clone()
+        ctx.codes, ctx.need_value = kcodes, need_value
+        ctx.save_for_backward(row, rowptr, col, value, colptr, csr2csc, mat, row_csc if need_mat else None,
+                              full if need else None, arg_min, arg_max)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row, rowptr, col, value, colptr, csr2csc, mat, row_csc, full, arg_min, arg_max = ctx.saved_tensors
+        need_value, need_mat = ctx.need_value, ctx.needs_input_grad[6]
+        if not (need_value or need_mat):
+            return None, None, None, None, None, None, None, None, None
+        codes = ctx.codes
+        acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
+
+        def grad_of(c: int) -> Optional[Tensor]:
+            return grad_out[:, codes.index(c)] if c in codes and codes.index(c) < grad_out.size(1) else None
+
+        # the row coefficients a and b are formed in fp32 (fp64) and rounded once to the dtype; the products and the
+        # sum of the gradient's terms run in the dtype, as autograd sums the terms of the unfused composition
+        dt = mat.dtype
+        g_sum, g_mean, g_var, g_std = grad_of(0), grad_of(1), grad_of(4), grad_of(5)
+        a = b = None
+        if g_mean is None and g_var is None and g_std is None:
+            a = g_sum
+        else:
+            inv_n = (rowptr[1:] - rowptr[:-1]).clamp(min=1).to(acc).reciprocal_().unsqueeze(1)
+            if g_mean is not None:
+                a = g_mean * inv_n
+            if g_sum is not None:
+                a = g_sum.to(acc, copy=True) if a is None else a.add_(g_sum)
+            gv = None   # g_v / n
+            if g_var is not None:
+                gv = (g_var * inv_n).masked_fill_(~(full[:, codes.index(4)] > 0), 0)
+            if g_std is not None:
+                std = full[:, codes.index(5)]
+                t = (g_std * inv_n).div_(std).mul_(0.5).masked_fill_(~(std > 0), 0)
+                gv = t if gv is None else gv.add_(t)
+            if gv is not None:
+                b = gv.mul_(2)
+                mb = b * full[:, codes.index(1)]
+                a = mb.neg_() if a is None else a.sub_(mb)
+                b = b.to(dt)
+            a = a.to(dt) if a is not None else None
+
+        grad_value = grad_mat = None
+        if need_mat:
+            if row_csc is None:
+                row_csc = row.index_select(0, csr2csc)
+            v_csc = value.index_select(0, csr2csc) if value is not None else None
+            if a is not None:
+                grad_mat = spmm_fw(colptr, row_csc, v_csc, a, "sum")[0]
+            if b is not None:
+                t = spmm_fw(colptr, row_csc, v_csc * v_csc if v_csc is not None else None, b, "sum")[0].mul_(mat)
+                grad_mat = t if grad_mat is None else grad_mat.add_(t)
+        if need_value:
+            if a is not None:
+                grad_value = spmm_value_bw(row, rowptr, col, mat, a, "sum")
+            if b is not None:
+                t = spmm_value_bw(row, rowptr, col, mat * mat, b, "sum").mul_(value)
+                grad_value = t if grad_value is None else grad_value.add_(t)
+        for c, arg in ((2, arg_min), (3, arg_max)):
+            g = grad_of(c)
+            if g is None:
+                continue
+            gvm, gmm = spmm_minmax_bw(col, value, mat, g, arg, need_value, need_mat)
+            if gvm is not None:
+                grad_value = gvm if grad_value is None else grad_value.add_(gvm)
+            if gmm is not None:
+                grad_mat = gmm if grad_mat is None else grad_mat.add_(gmm)
+        if need_mat and grad_mat is None:
+            grad_mat = torch.zeros_like(mat)
+        if need_value and grad_value is None:
+            grad_value = torch.zeros_like(value)
+        return None, None, None, grad_value, None, None, grad_mat, None, None
+
+
+def spmm_multi(row: Optional[Tensor], rowptr: Tensor, col: Tensor, value: Optional[Tensor], colptr: Optional[Tensor],
+               csr2csc: Optional[Tensor], mat: Tensor, row_csc: Optional[Tensor], aggrs: List[str]) -> Tensor:
+    return SPMMMulti.apply(row, rowptr, col, value, colptr, csr2csc, mat, row_csc, aggrs)
 
 
 def _minmax_forward(ctx, reduce, rowptr, col, value, mat):

@@ -25,7 +25,8 @@ INCLUDE = ROOT / "include"
 BUILD = CSRC / "_build"
 LIB = PKG / "libtsb200.so"
 
-SOURCES = ["spmm_fw.cu", "spmm_bw.cu", "convert.cu", "coalesce.cu", "spspmm.cu", "quant.cu", "softmax.cu", "host_api.cu"]
+SOURCES = ["spmm_fw.cu", "spmm_softmax_aggr.cu", "spmm_bw.cu", "convert.cu", "coalesce.cu", "spspmm.cu", "quant.cu",
+           "softmax.cu", "host_api.cu"]
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [

@@ -239,6 +239,64 @@ TSB200_API int tsb200_spmm_fw_multi(const int64_t* rowptr, const int64_t* col, c
                                     size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Softmax-aggregation SpMM: per row m and column k the messages p_e = value[e] * mat[col[e], k] weighted by a softmax
+ * over the row's entries with a temperature t_k, as GENConv's softmax aggregation (no counterpart in the reference).
+ * B = 1. With A the accumulator type (fp32; fp64 for F64):
+ *     p_e = fl_A(v_e x[col_e, k])   (exact for F16 / BF16),   y_e = fl_A(t_k p_e)
+ *     mu = max_e y_e,   w_e = exp(y_e - mu),   s = sum_e w_e,   a = sum_e w_e p_e
+ *     out[m, k] = round(a / s)  (one IEEE division),   lse[m, k] = mu + log(s)  (type A)
+ *   Every stored entry counts, duplicates included. An empty row gives out = +0 and lse = -inf. NaN in x, value or t
+ *   propagates to the columns it reaches. Inputs whose t * p is not finite are outside this contract: they do not
+ *   fault, and give NaN or an unspecified value. The kernels run the softmax online (rescaling s and a when mu
+ *   grows); the fp32 exp is ex2.approx.ftz of a log2(e)-scaled argument (exp(0) = 1, exp(-inf) = +0). With t = 0 the
+ *   result is bit for bit tsb200_spmm_fw / _planned MEAN on the same path and work-item size for F16 / BF16, and for
+ *   F32 without values. A one-entry row gives round(p). Negative t is allowed (a soft minimum).
+ *   mat dtype[N, K], value dtype[E] or NULL (1), t type A with t_stride 0 (one scalar) or 1 (one per column, [K]),
+ *   out dtype[M, K], lse A[M, K] or NULL (not stored). dtype F32 / F64 / F16 / BF16.
+ *   plan == NULL: workspace tsb200_spmm_fw_softmax_aggr_workspace_bytes(K, E, 0, 0, 0). Otherwise `plan` is a
+ *   tsb200_spmm_plan of rowptr with its counts, workspace tsb200_spmm_fw_softmax_aggr_workspace_bytes(K, E, 1, n_long,
+ *   n_slot). Both are read on the vector path only (F32 / F16 / BF16, K * sizeof(dtype) % 16 == 0, E > 0, the extents
+ *   and alignments of tsb200_spmm_fw, lse 16-byte aligned); any other call runs the generic kernel, which reads neither.
+ *   TSB200_ERR_INVALID_ARG for a negative extent or count, a NULL pointer that is needed or t_stride not 0 / 1;
+ *   TSB200_ERR_UNSUPPORTED for an integer dtype or a t not aligned to its element size; TSB200_ERR_WORKSPACE for a
+ *   missing or short workspace.
+ *
+ * Its backward. With g = grad_out, o = out and l = lse (the forward's) of row r, and alpha_e = exp(t p_e - l), the
+ * gradient of message e is d_e = g alpha_e (1 + t (p_e - o)), per column.
+ *   tsb200_spmm_softmax_aggr_bw_rows: grad_value[e] = <x[col_e], d_e> (dtype[E], needs value) and
+ *     U[r, k] = g[r, k] sum_{e in row r} alpha_e (p_e - o[r, k])^2 (type A [M, K]; the temperature's gradient is
+ *     U.sum(0), or U.sum() for one scalar). Either output may be NULL: it is not wanted.
+ *   tsb200_spmm_softmax_aggr_bw_cols: grad_mat[n] = sum_{e in column n} v_e d_e (dtype[N, K]), on the CSC view:
+ *     colptr[N + 1], row_csc[E] and value_csc = value[csr2csc] (or NULL) in place of rowptr, col and value. grad_mat
+ *     NULL: nothing is launched.
+ *   F32 / F16 / BF16 rows of 16 ... 1024 bytes (K * sizeof(dtype) a multiple of 16), E > 0, the extents of
+ *   tsb200_spmm_fw and 16-byte aligned mat, grad_out, out, lse (and grad_mat) run row-split kernels: rows (columns)
+ *   longer than 256 entries, or past a 32-row item's budget, are cut into segments whose fp32 partials are summed in
+ *   segment order. They need workspace tsb200_spmm_softmax_aggr_bw_workspace_bytes(K, E), 256-byte aligned (one
+ *   workspace serves either call). Any other call runs a generic kernel (a warp per row or column, a lane per feature
+ *   column) and reads no workspace. No atomics: every gradient is the same bit for bit from run to run. Return codes
+ *   as the forward's.
+ * ------------------------------------------------------------------------------------------ */
+TSB200_API size_t tsb200_spmm_fw_softmax_aggr_workspace_bytes(int64_t K, int64_t E, int planned, int64_t n_long,
+                                                              int64_t n_slot);
+TSB200_API int tsb200_spmm_fw_softmax_aggr(const int64_t* rowptr, const int64_t* col, const void* value,
+                                           const void* mat, const void* t, int64_t t_stride, void* out, void* lse,
+                                           int64_t M, int64_t N, int64_t K, int64_t E, int dtype, const void* plan,
+                                           size_t plan_bytes, int64_t n_seg, int64_t n_long, int64_t n_slot,
+                                           void* workspace, size_t workspace_bytes, void* stream);
+TSB200_API int tsb200_spmm_softmax_aggr_bw_rows(const int64_t* rowptr, const int64_t* col, const void* value,
+                                                const void* mat, const void* t, int64_t t_stride, const void* grad_out,
+                                                const void* out, const void* lse, void* grad_value, void* U, int64_t M,
+                                                int64_t N, int64_t K, int64_t E, int dtype, void* workspace,
+                                                size_t workspace_bytes, void* stream);
+TSB200_API int tsb200_spmm_softmax_aggr_bw_cols(const int64_t* colptr, const int64_t* row_csc, const void* value_csc,
+                                                const void* mat, const void* t, int64_t t_stride, const void* grad_out,
+                                                const void* out, const void* lse, void* grad_mat, int64_t M, int64_t N,
+                                                int64_t K, int64_t E, int dtype, void* workspace,
+                                                size_t workspace_bytes, void* stream);
+TSB200_API size_t tsb200_spmm_softmax_aggr_bw_workspace_bytes(int64_t K, int64_t E);
+
+/* ------------------------------------------------------------------------------------------
  * FP8 (e4m3) quantisation of a float matrix: the operand of tsb200_spmm_fw_fp8, made without float temporaries (no
  * counterpart in the reference).
  *   x dtype[N, K] with dtype in {F32, F16, BF16}, row m at x + m * ld elements (ld >= K; the last dimension is

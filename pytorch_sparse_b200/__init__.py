@@ -13,7 +13,7 @@ from .storage import SparseStorage  # noqa: F401
 from .tensor import SparseTensor  # noqa: F401
 from .matmul import matmul, spmm_sum, spmm_add, spmm_mean, spmm_min, spmm_max, spspmm_sum  # noqa: F401
 from .matmul import spmm_fp8, spmm_fp8_quant, quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads  # noqa: F401
-from .matmul import spmm_multi  # noqa: F401
+from .matmul import spmm_multi, spmm_softmax_aggr  # noqa: F401
 from .softmax import softmax  # noqa: F401
 from .transpose import t, transpose  # noqa: F401
 from .functional import coalesce, spmm, spspmm  # noqa: F401
@@ -25,7 +25,8 @@ from . import torch_ops  # noqa: F401  (registers torch.ops.tsb200.* / torch.ops
 __version__ = "0.1.0"
 
 __all__ = ["SparseStorage", "SparseTensor", "t", "matmul", "coalesce", "transpose", "spmm", "spspmm", "spmm_fp8",
-           "spmm_fp8_quant", "quantize_fp8", "sddmm", "sddmm_fp8", "spmm_heads", "sddmm_heads", "spmm_multi", "softmax",
+           "spmm_fp8_quant", "quantize_fp8", "sddmm", "sddmm_fp8", "spmm_heads", "sddmm_heads", "spmm_multi",
+           "spmm_softmax_aggr", "softmax",
            "spadd",
            "add",
            "add_", "add_nnz", "add_nnz_",

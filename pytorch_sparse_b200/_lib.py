@@ -47,6 +47,17 @@ SIGNATURES = {
     "tsb200_spmm_fw_multi": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                      c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t,
                                      c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_fw_softmax_aggr_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int64, c_int64]),
+    "tsb200_spmm_fw_softmax_aggr": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                            c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t,
+                                            c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_softmax_aggr_bw_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
+                                                 c_int64, c_int, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_softmax_aggr_bw_cols": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                                 c_int, c_void_p, c_size_t, c_void_p]),
+    "tsb200_spmm_softmax_aggr_bw_workspace_bytes": (c_size_t, [c_int64, c_int64]),
     "tsb200_quantize_fp8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_size_t, c_void_p]),
     "tsb200_spmm_fw_acc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

@@ -511,4 +511,207 @@ static inline int warp_grid(int64_t n_warps, int cap_per_sm) {
   return (int)min((n_warps + 7) / 8, (int64_t)num_sms() * cap_per_sm);
 }
 
+// ---- the row-split kernels' building blocks: value loads, the engine hooks, the segment queue, the work-item
+// front, a lane's columns, the segment walk, and on the host the plan and planned-workspace layouts. The SpMM
+// forward (spmm_fw.cu) and the softmax aggregation (spmm_softmax_aggr.cu) both build their kernels from these.
+template <typename T> __device__ __forceinline__ typename Vec<T>::vraw load_vraw(const T* p);
+template <> __device__ __forceinline__ float load_vraw<float>(const float* p) { return __ldg(p); }
+template <> __device__ __forceinline__ unsigned short load_vraw<__nv_bfloat16>(const __nv_bfloat16* p) {
+  return __ldg(reinterpret_cast<const unsigned short*>(p));
+}
+template <> __device__ __forceinline__ unsigned short load_vraw<__half>(const __half* p) {
+  return __ldg(reinterpret_cast<const unsigned short*>(p));
+}
+
+template <typename Eng> __device__ __forceinline__ void set_scale(Eng& eng, const SpmmParams& p) {
+  if constexpr (Eng::Q8) {
+    eng.scale = p.scale;
+    eng.sstride = p.scale_stride;
+  }
+}
+// HEADS: the head of each of this lane's chunks (chunk ch starts at column k0 + (ch * LPR + li) * VEC), computed once
+// per kernel by head_cols, and handed to every row's engine by set_heads
+template <bool HEADS, int LPR, int VEC, int CH>
+__device__ __forceinline__ void head_cols(int (&hcol)[HEADS ? CH : 1], const SpmmParams& p, int li) {
+  if constexpr (HEADS) {
+    const int D = (int)(p.K / p.heads);
+#pragma unroll
+    for (int ch = 0; ch < CH; ch++) hcol[ch] = (p.k0 + (ch * LPR + li) * VEC) / D;
+  }
+}
+template <bool HEADS, typename Eng, int NH>
+__device__ __forceinline__ void set_heads(Eng& eng, const SpmmParams& p, const int (&hcol)[NH]) {
+  if constexpr (HEADS) {
+    eng.hval = (decltype(eng.hval))p.value;
+    eng.heads = p.heads;
+#pragma unroll
+    for (int i = 0; i < NH; i++) eng.hcol[i] = hcol[i];
+  }
+}
+
+// queue a row deferred by defer_row (row r0 + lane of batch b, nnz [rp0, rp1), deg = rp1 - rp0) as segments of
+// <= kSeg nnz; a row of several segments also gets a LongRow and one partial slot per segment, for the combine
+__device__ __forceinline__ void push_row_segments(const SpmmParams& p, int64_t b, int64_t r0, int lane, int64_t rp0,
+                                                  int64_t rp1, int deg) {
+  const int nseg = (deg + kSeg - 1) / kSeg;
+  const unsigned seg0 = atomicAdd(&p.counters[1], (unsigned)nseg);
+  int64_t slot0 = -1;
+  if (nseg > 1) {
+    slot0 = atomicAdd(&p.counters[3], (unsigned)nseg);
+    const unsigned lr = atomicAdd(&p.counters[2], 1u);
+    if ((int64_t)lr < p.long_cap) {
+      LongRow L;
+      L.row_b = b * p.M + r0 + lane;
+      L.first_slot = slot0;
+      L.nseg_count = ((int64_t)nseg << 40) | (int64_t)deg;
+      p.longs[lr] = L;
+    }
+  }
+  for (int sgi = 0; sgi < nseg; sgi++) {
+    if ((int64_t)seg0 + sgi < p.seg_cap) {
+      Segment S;
+      S.row_b = b * p.M + r0 + lane;
+      S.start = rp0 + (int64_t)sgi * kSeg;
+      S.end = min(rp1, S.start + kSeg);
+      S.slot = slot0 < 0 ? -1 : slot0 + sgi;
+      p.segs[seg0 + sgi] = S;
+    }
+  }
+}
+
+// ---- the front of a main kernel's work items ------------------------------------------------------
+// A warp takes tickets from p.counters[0]; start() takes the next one as an item starts, so that the atomic's latency
+// hides behind the item. Ticket t is row block t % nblk of batch b = t / nblk: rows [r0, r0 + nrows), 2^item_shift of
+// them but fewer at the end. Lane l holds the nnz range [rp0, rp1) of row r0 + l (lanes >= nrows: the item's end).
+//   for (WorkItem it(p, lane); it.start(p, lane); it.advance()) { ... }
+struct WorkItem {
+  int item_rows;
+  int64_t nblk, n_items;
+  unsigned int ticket, next_ticket;
+  int64_t b, r0, rp0, rp1;
+  int nrows;
+
+  __device__ __forceinline__ WorkItem(const SpmmParams& p, int lane) {
+    item_rows = 1 << p.item_shift;
+    nblk = (p.M + item_rows - 1) >> p.item_shift;
+    n_items = nblk * p.B;
+    ticket = __shfl_sync(0xffffffffu, take_ticket(&p.counters[0], lane), 0);
+  }
+  __device__ __forceinline__ bool start(const SpmmParams& p, int lane) {
+    if ((int64_t)ticket >= n_items) return false;
+    next_ticket = take_ticket(&p.counters[0], lane);
+    b = ticket / nblk;
+    r0 = (ticket - b * nblk) << p.item_shift;
+    nrows = (int)min((int64_t)item_rows, p.M - r0);
+    rp0 = __ldg(p.rowptr + r0 + min(lane, nrows));
+    rp1 = __ldg(p.rowptr + r0 + min(lane + 1, nrows));
+    return true;
+  }
+  __device__ __forceinline__ void advance() { ticket = __shfl_sync(0xffffffffu, next_ticket, 0); }
+  // planned kernels: the item's rows in the segment list, bit r of plan_mask[r / 32], clipped to nrows
+  __device__ __forceinline__ unsigned plan_defer_mask(const SpmmParams& p) const {
+    const uint32_t w = __ldg(p.plan_mask + (r0 >> 5));
+    return (w >> (r0 & 31)) & (nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u));
+  }
+};
+
+// ---- a lane's columns in the row-per-warp kernels ---------------------------------------------------
+// Chunk ch of lane li starts at column k0 + (ch * LPR + li) * VEC; col_ok[ch]: it lies inside the row. row_bytes is
+// one dense row, lane_off the byte offset of the lane's first column in it, hcol (HEADS) the head of each chunk.
+template <typename X, int LPR, int VEC, int CH, bool HEADS>
+__device__ __forceinline__ void lane_cols(const SpmmParams& p, int li, bool (&col_ok)[CH], int (&hcol)[HEADS ? CH : 1],
+                                          uint32_t& row_bytes, int64_t& lane_off) {
+#pragma unroll
+  for (int ch = 0; ch < CH; ch++) col_ok[ch] = p.k0 + (ch * LPR + li) * VEC < p.K;
+  head_cols<HEADS, LPR, VEC, CH>(hcol, p, li);
+  row_bytes = (uint32_t)(p.K * (int64_t)sizeof(X));
+  lane_off = ((int64_t)p.k0 + (int64_t)li * VEC) * (int64_t)sizeof(X);
+}
+
+// walk segment S (of batch b; B == 1 in the planned drain) with the row engine eng, which then holds the segment's
+// result in every lane group. The segment kernel and the planned drain both walk segments here, which is what makes
+// planned and unplanned products agree on the rows they defer. Each finishes a segment itself, in its own branch
+// order (the order decides their machine code): the row store for a whole row, else the fp32 partial.
+template <bool HEADS, typename Eng, typename T, int CH, int NH>
+__device__ __forceinline__ void walk_segment(Eng& eng, const SpmmParams& p, const Segment& S, int64_t b,
+                                             IndexRing<T>& ring, const bool (&col_ok)[CH], const int (&hcol)[NH],
+                                             uint32_t row_bytes, int64_t lane_off, int lane, int g, uint64_t pol) {
+  const int64_t base = S.start & ~(int64_t)31;
+  ring.reset(base, S.end);
+  const char* matb = (const char*)p.mat + b * p.N * (int64_t)row_bytes + lane_off;
+  asm volatile("" : "+l"(matb));
+  eng.init();
+  set_scale(eng, p);
+  set_heads<HEADS>(eng, p, hcol);
+  eng.accumulate(ring, (int)(S.start - base), (int)(S.end - base), matb, row_bytes, col_ok, lane, g, pol);
+  eng.reduce_groups();
+}
+
+struct PlanLayout {
+  size_t header, mask, segs, seg_lr, longs, total;
+  int64_t seg_cap, long_cap;
+};
+static inline PlanLayout plan_layout(int64_t M, int64_t E) {
+  PlanLayout L;
+  const WsLayout W = ws_layout(1, 1, E, false, false);
+  L.seg_cap = W.seg_cap;
+  L.long_cap = W.long_cap;
+  size_t off = 0;
+  L.header = off; off += 256;
+  L.mask = off; off += align_up((size_t)((M + 31) / 32 + 1) * 4, 256);
+  L.segs = off; off += align_up((size_t)L.seg_cap * sizeof(Segment), 256);
+  L.seg_lr = off; off += align_up((size_t)L.seg_cap * 4, 256);
+  L.longs = off; off += align_up((size_t)L.long_cap * sizeof(LongRow), 256);
+  L.total = off;
+  return L;
+}
+struct PlannedWs {
+  size_t counters, long_done, part_val, part_arg, total;
+};
+static inline PlannedWs planned_ws(int64_t K, int64_t n_long, int64_t n_slot, bool arg) {
+  PlannedWs L;
+  size_t off = 0;
+  L.counters = off; off += 256;
+  L.long_done = off; off += align_up((size_t)(n_long > 0 ? n_long : 1) * 4, 256);
+  L.part_val = off; off += align_up((size_t)(n_slot > 0 ? n_slot : 1) * (size_t)K * sizeof(float), 256);
+  L.part_arg = off; off += arg ? align_up((size_t)(n_slot > 0 ? n_slot : 1) * (size_t)K * sizeof(int64_t), 256) : 0;
+  L.total = off;
+  return L;
+}
+// checks a plan of p.M rows and p.E nnz (tsb200_spmm_plan, with its counts) and its planned workspace, then binds
+// both to p: 0 or the error code
+static inline int bind_plan(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                     int64_t n_slot, void* workspace, size_t workspace_bytes, bool arg) {
+  const PlanLayout PL = plan_layout(p.M, p.E);
+  if (plan_bytes < PL.total) return TSB200_ERR_WORKSPACE;
+  if (n_seg > PL.seg_cap || n_long > PL.long_cap || ((uintptr_t)plan & 255)) return TSB200_ERR_INVALID_ARG;
+  const PlannedWs W = planned_ws(p.K, n_long, n_slot, arg);
+  if (!workspace || workspace_bytes < W.total) return TSB200_ERR_WORKSPACE;
+  if ((uintptr_t)workspace & 255) return TSB200_ERR_INVALID_ARG;
+  char* ws = (char*)workspace;
+  const char* pl = (const char*)plan;
+  p.counters = (unsigned int*)(ws + W.counters);
+  p.long_done = (uint32_t*)(ws + W.long_done);   // directly behind the counters: one memset clears both
+  p.segs = (Segment*)(pl + PL.segs);
+  p.longs = (LongRow*)(pl + PL.longs);
+  p.seg_lr = (const uint32_t*)(pl + PL.seg_lr);
+  p.plan_mask = (const uint32_t*)(pl + PL.mask);
+  p.n_seg = n_seg; p.n_long = n_long;
+  p.part_val = ws + W.part_val;
+  p.part_arg = arg ? (int64_t*)(ws + W.part_arg) : nullptr;
+  p.seg_cap = PL.seg_cap; p.long_cap = PL.long_cap; p.slot_cap = n_slot;
+  return 0;
+}
+// a plan and its planned workspace, or else an unplanned workspace: 0 or the error code
+static inline int bind_workspace(SpmmParams& p, const void* plan, size_t plan_bytes, int64_t n_seg, int64_t n_long,
+                          int64_t n_slot, void* workspace, size_t workspace_bytes, bool arg) {
+  return plan ? bind_plan(p, plan, plan_bytes, n_seg, n_long, n_slot, workspace, workspace_bytes, arg)
+              : bind_unplanned(p, workspace, workspace_bytes, arg);
+}
+
+__device__ __forceinline__ void long_row_counts(const LongRow& L, int& nseg, int64_t& count) {
+  nseg = (int)(L.nseg_count >> 40);
+  count = L.nseg_count & (((int64_t)1 << 40) - 1);
+}
+
 }  // namespace tsb

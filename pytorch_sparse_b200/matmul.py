@@ -141,6 +141,35 @@ def spmm_multi(src: SparseTensor, other: Tensor, aggrs: List[str]) -> Tensor:
     return torch.ops.tsb200.spmm_multi(row, rowptr, col, value, colptr, csr2csc, other, row_csc, aggrs)
 
 
+def spmm_softmax_aggr(src: SparseTensor, other: Tensor, t: Optional[Tensor] = None) -> Tensor:
+    """Softmax aggregation of every row's messages p_e = value[e] * other[col[e]], per feature column k:
+    out[m, k] = sum_e softmax_e(t_k p_e) p_e over the entries of row m, as PyG's SoftmaxAggregation and GENConv's
+    default aggregation compute it, in one gather pass with no [E, K] temporary. `other` is 2-D [N, K] (bf16, f16,
+    f32, f64); `t` is the temperature in float32 (float64 for f64) of shape [] or [1] (one for all columns) or [K], or
+    None for t = 1 (not learnable). The softmax runs online in fp32 (fp64), shifted by each row's own maximum, so rows
+    far from the column's global maximum do not underflow. An empty row gives 0; t = 0 gives `spmm(src, other,
+    "mean")`, and a negative t a soft minimum. Differentiable in the values, `other` and `t`; only a gradient to
+    `other` builds the CSC view."""
+    if other.dim() != 2:
+        raise RuntimeError("spmm_softmax_aggr: other must be 2-D [N, K], got " + str(other.dim()) + "-D")
+    N = src.size(1)
+    if other.size(0) != N:
+        raise RuntimeError("spmm_softmax_aggr: other must have " + str(N) + " rows (the sparse sizes), got "
+                           + str(other.size(0)))
+    rowptr, col, value = src.csr()
+    st = src.storage
+    colptr: Optional[Tensor] = None
+    csr2csc: Optional[Tensor] = None
+    row_csc: Optional[Tensor] = None
+    if value is not None:
+        value = value.to(other.dtype)
+    if other.requires_grad:     # the column-wise backward runs on the CSC view
+        csr2csc = st.csr2csc()
+        colptr = st.colptr()
+        row_csc = st.row_csc()
+    return torch.ops.tsb200.spmm_softmax_aggr(rowptr, col, value, colptr, csr2csc, other, row_csc, t)
+
+
 def spmm_fp8(src: SparseTensor, x8: Tensor, scale: Tensor, reduce: str = "sum",
              out_dtype: torch.dtype = torch.bfloat16, residual: Optional[Tensor] = None,
              residual_scale: Optional[Tensor] = None) -> Tensor:
@@ -348,6 +377,7 @@ SparseTensor.sddmm_fp8 = lambda self, a8, a_scale, b8, b_scale, out_dtype=torch.
     self, a8, a_scale, b8, b_scale, out_dtype)
 SparseTensor.spmm_heads = lambda self, x: spmm_heads(self, x)
 SparseTensor.spmm_multi = lambda self, other, aggrs: spmm_multi(self, other, aggrs)
+SparseTensor.spmm_softmax_aggr = lambda self, other, t=None: spmm_softmax_aggr(self, other, t)
 SparseTensor.sddmm_heads = lambda self, a, b: sddmm_heads(self, a, b)
 SparseTensor.spspmm = lambda self, other, reduce="sum": spspmm(self, other, reduce)
 SparseTensor.matmul = lambda self, other, reduce="sum": matmul(self, other, reduce)

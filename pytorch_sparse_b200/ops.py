@@ -382,6 +382,126 @@ def spmm_fw_multi(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Ten
     return _spmm_fw_multi(rowptr, col, value, mat, _aggr_codes(aggrs), want_args, plan)
 
 
+def _smx_t(t: Tensor, mat: Tensor) -> int:
+    """The checks of a softmax aggregation's temperature; returns its stride (0: one scalar, 1: one per column)."""
+    _check_cuda(t, "t")
+    acc = torch.float64 if mat.dtype == torch.float64 else torch.float32
+    if t.device != mat.device:
+        raise RuntimeError(f"spmm_softmax_aggr: t must be on the device of the dense operand ({mat.device})")
+    if t.dtype != acc:
+        raise RuntimeError(f"spmm_softmax_aggr: t must be {acc} for a {mat.dtype} operand, got {t.dtype}")
+    K = mat.size(-1)
+    if t.dim() == 0 or (t.dim() == 1 and t.size(0) == 1):
+        return 0
+    if t.dim() == 1 and t.size(0) == K:
+        return 1
+    raise RuntimeError(f"spmm_softmax_aggr: t must have shape [], [1] or [K] = [{K}], got {list(t.shape)}")
+
+
+def _smx_operands(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor):
+    _check_cuda(rowptr, "rowptr")
+    _check_cuda(col, "col")
+    if value is not None:
+        _check_cuda(value, "optional_value.value()")
+    _check_cuda(mat, "mat")
+    if mat.dim() != 2:
+        raise RuntimeError(f"spmm_softmax_aggr: the dense operand must be 2-D [N, K], got {mat.dim()}-D")
+    _check_input(rowptr.dim() == 1)
+    _check_input(col.dim() == 1)
+    if value is not None:
+        _check_input(value.dim() == 1)
+        _check_input(value.size(0) == col.size(0))
+        if value.dtype != mat.dtype:
+            raise RuntimeError(f"expected value of dtype {mat.dtype} but got {value.dtype}")
+        value = value.contiguous()
+    return _i64(rowptr, "rowptr"), _i64(col, "col"), value, mat.contiguous()
+
+
+def spmm_fw_softmax_aggr(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, t: Tensor,
+                         want_lse: bool = False,
+                         plan: Optional[SpmmPlan] = None) -> Tuple[Tensor, Optional[Tensor]]:
+    """`(out [M, K], lse [M, K]?)`: per row m and column k the messages p_e = value[e] * mat[col[e], k] summed with
+    the weights softmax_e(t_k p_e) over the row's entries (tsb200_spmm_fw_softmax_aggr), and lse = max_e t_k p_e +
+    log(sum_e exp(t_k p_e - max)) in fp32 (fp64 for f64) when want_lse. `mat` is 2-D [N, K] (bf16, f16, f32, f64); `t`
+    has the accumulator dtype (float32, float64 for f64) and shape [] or [1] (one temperature) or [K] (one per column).
+    An empty row gives 0 (lse -inf). With t = 0 the result is bit for bit `spmm_fw(..., "mean")` on the same path for
+    bf16 / f16, and for f32 without values. Planned like `spmm_fw` (the same per-rowptr plan cache). Forward only: see
+    SPMMSoftmaxAggr."""
+    rowptr, col, value, mat = _smx_operands(rowptr, col, value, mat)
+    stride = _smx_t(t, mat)
+    t = t.contiguous()
+    dt = _dtype_code(mat.dtype)
+    M = rowptr.numel() - 1
+    N, K = mat.shape
+    E = col.numel()
+    dev = mat.device
+    out = torch.empty(M, K, dtype=mat.dtype, device=dev)
+    lse = torch.empty(M, K, dtype=t.dtype, device=dev) if want_lse else None
+    if out.numel() == 0:
+        return out, lse
+    with _on_device(dev):
+        plannable = E > 0 and dt in (0, 2, 3) and (K * mat.element_size()) % 16 == 0
+        if plannable and plan is None:
+            plan = _auto_plan(rowptr, E)
+        if plannable and plan is not None and plan.M == M and plan.E == E:
+            nws = lib.tsb200_spmm_fw_softmax_aggr_workspace_bytes(K, E, 1, plan.n_long, plan.n_slot)
+            pl = (_p(plan.data), plan.data.numel(), plan.n_seg, plan.n_long, plan.n_slot)
+        else:
+            nws = lib.tsb200_spmm_fw_softmax_aggr_workspace_bytes(K, E, 0, 0, 0)
+            pl = (None, 0, 0, 0, 0)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_fw_softmax_aggr(_p(rowptr), _p(col), _p(value), _p(mat), _p(t), stride, _p(out),
+                                              _p(lse), M, N, K, E, dt, *pl, _p(ws), nws, _stream(dev)),
+              "tsb200_spmm_fw_softmax_aggr")
+    return out, lse
+
+
+def spmm_softmax_aggr_bw_rows(rowptr: Tensor, col: Tensor, value: Optional[Tensor], mat: Tensor, t: Tensor,
+                              grad_out: Tensor, out: Tensor, lse: Tensor, want_value: bool,
+                              want_t: bool) -> Tuple[Optional[Tensor], Optional[Tensor]]:
+    """The row-wise backward of `spmm_fw_softmax_aggr` (tsb200_spmm_softmax_aggr_bw_rows): `(grad_value [E]?, U
+    [M, K]?)` with U[r, k] = g[r, k] sum_e alpha_e (p_e - out[r, k])^2 in t's dtype, whose column sums are the
+    temperature's gradient."""
+    rowptr, col, value, mat = _smx_operands(rowptr, col, value, mat)
+    stride = _smx_t(t, mat)
+    M = rowptr.numel() - 1
+    N, K = mat.shape
+    E = col.numel()
+    dev = mat.device
+    gv = torch.empty(E, dtype=mat.dtype, device=dev) if want_value and value is not None else None
+    U = torch.empty(M, K, dtype=t.dtype, device=dev) if want_t else None
+    with _on_device(dev):
+        nws = lib.tsb200_spmm_softmax_aggr_bw_workspace_bytes(K, E)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_softmax_aggr_bw_rows(_p(rowptr), _p(col), _p(value), _p(mat), _p(t.contiguous()),
+                                                   stride, _p(grad_out.contiguous()), _p(out), _p(lse), _p(gv), _p(U),
+                                                   M, N, K, E, _dtype_code(mat.dtype), _p(ws), nws, _stream(dev)),
+              "tsb200_spmm_softmax_aggr_bw_rows")
+    return gv, U
+
+
+def spmm_softmax_aggr_bw_cols(colptr: Tensor, row_csc: Tensor, value_csc: Optional[Tensor], mat: Tensor, t: Tensor,
+                              grad_out: Tensor, out: Tensor, lse: Tensor) -> Tensor:
+    """The column-wise backward of `spmm_fw_softmax_aggr` (tsb200_spmm_softmax_aggr_bw_cols) on the CSC view:
+    grad_mat [N, K]."""
+    colptr, row_csc, value_csc, mat = _smx_operands(colptr, row_csc, value_csc, mat)
+    stride = _smx_t(t, mat)
+    N, K = mat.shape
+    M = out.size(0)
+    E = row_csc.numel()
+    dev = mat.device
+    grad_mat = torch.empty_like(mat)
+    with _on_device(dev):
+        nws = lib.tsb200_spmm_softmax_aggr_bw_workspace_bytes(K, E)
+        ws = _workspace(nws, dev)
+        check(lib.tsb200_spmm_softmax_aggr_bw_cols(_p(colptr), _p(row_csc), _p(value_csc), _p(mat),
+                                                   _p(t.contiguous()), stride, _p(grad_out.contiguous()), _p(out),
+                                                   _p(lse), _p(grad_mat), M, N, K, E, _dtype_code(mat.dtype), _p(ws),
+                                                   nws, _stream(dev)),
+              "tsb200_spmm_softmax_aggr_bw_cols")
+    return grad_mat
+
+
 _FP8_OUT = {torch.float32: 0, torch.float16: 2, torch.bfloat16: 3}
 
 
@@ -1393,6 +1513,59 @@ class SPMMMulti(torch.autograd.Function):
 def spmm_multi(row: Optional[Tensor], rowptr: Tensor, col: Tensor, value: Optional[Tensor], colptr: Optional[Tensor],
                csr2csc: Optional[Tensor], mat: Tensor, row_csc: Optional[Tensor], aggrs: List[str]) -> Tensor:
     return SPMMMulti.apply(row, rowptr, col, value, colptr, csr2csc, mat, row_csc, aggrs)
+
+
+class SPMMSoftmaxAggr(torch.autograd.Function):
+    """`spmm_fw_softmax_aggr`, differentiable in the values, `mat` and `t`. With g = grad_out, o = out and
+    alpha_e = exp(t p_e - lse), the gradient of message e is d_e = g alpha_e (1 + t (p_e - o)), per column:
+        grad_value[e] = <x[col_e], d_e>,  grad_t = sum_r g[r] sum_{e in r} alpha_e (p_e - o[r])^2   (row-wise kernel)
+        grad_mat[n] = sum_{e in column n} v_e d_e                                             (column-wise kernel)
+    out and lse are saved only when a gradient is wanted, only the kernels whose gradients are wanted run, and only
+    grad_mat reads the CSC view (colptr, csr2csc, row_csc). grad_t is U.sum(0) (U.sum() for one temperature) of the
+    kernel's per-row plane, with no atomics anywhere, so it is the same bit for bit from run to run."""
+    @staticmethod
+    def forward(ctx, rowptr, col, value, colptr, csr2csc, mat, row_csc, t):
+        need_value = value is not None and ctx.needs_input_grad[2]
+        need_mat = ctx.needs_input_grad[5]
+        need_t = t is not None and ctx.needs_input_grad[7]
+        if need_mat:
+            _assert_present(colptr, "colptr")
+            _assert_present(csr2csc, "csr2csc")
+        if t is None:   # t = 1, not learnable
+            key = (mat.device, torch.float64 if mat.dtype == torch.float64 else torch.float32)
+            t = _ONE.get(key)
+            if t is None:
+                t = _ONE[key] = torch.ones((), dtype=key[1], device=mat.device)
+        need = need_value or need_mat or need_t
+        out, lse = spmm_fw_softmax_aggr(rowptr, col, value, mat, t, want_lse=need)
+        ctx.need = (need_value, need_mat, need_t)
+        ctx.save_for_backward(rowptr, col, value, colptr, csr2csc, mat, row_csc if need_mat else None, t,
+                              out if need else None, lse)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        rowptr, col, value, colptr, csr2csc, mat, row_csc, t, out, lse = ctx.saved_tensors
+        need_value, need_mat, need_t = ctx.need
+        grad_value = grad_mat = grad_t = None
+        grad_out = grad_out.contiguous()
+        if need_value or need_t:
+            grad_value, U = spmm_softmax_aggr_bw_rows(rowptr, col, value, mat, t, grad_out, out, lse, need_value,
+                                                      need_t)
+            if U is not None:
+                grad_t = (U.sum(0) if t.dim() == 1 and t.numel() > 1 else U.sum()).reshape(t.shape)
+        if need_mat:
+            if row_csc is None:
+                row_csc = ptr2ind(rowptr, col.numel()).index_select(0, csr2csc)
+            v_csc = value.index_select(0, csr2csc) if value is not None else None
+            grad_mat = spmm_softmax_aggr_bw_cols(colptr, row_csc, v_csc, mat, t, grad_out, out, lse)
+        return None, None, grad_value, None, None, grad_mat, None, grad_t
+
+
+def spmm_softmax_aggr(rowptr: Tensor, col: Tensor, value: Optional[Tensor], colptr: Optional[Tensor],
+                      csr2csc: Optional[Tensor], mat: Tensor, row_csc: Optional[Tensor],
+                      t: Optional[Tensor]) -> Tensor:
+    return SPMMSoftmaxAggr.apply(rowptr, col, value, colptr, csr2csc, mat, row_csc, t)
 
 
 def _minmax_forward(ctx, reduce, rowptr, col, value, mat):

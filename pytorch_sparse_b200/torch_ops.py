@@ -3,7 +3,8 @@
 
     torch.ops.tsb200.{spmm_sum, spmm_mean, spmm_min, spmm_max, ind2ptr, ptr2ind, cuda_version}
     torch.ops.tsb200.{coalesce, sort_perm, csr2csc, segment_reduce, spspmm, spmm_res, spmm_fp8, spmm_fp8_quant,
-                      quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads, spmm_multi, segment_softmax}  (own)
+                      quantize_fp8, sddmm, sddmm_fp8, spmm_heads, sddmm_heads, spmm_multi, spmm_softmax_aggr,
+                      segment_softmax}  (own)
 
 and — unless a `torch_sparse` package is importable in this environment or TSB200_REGISTER_TORCH_SPARSE=0 —
 the same operators as `torch.ops.torch_sparse.*`, so code that calls the reference's ops by name
@@ -62,6 +63,9 @@ _EXTRA_SCHEMAS = {
     # several aggregations (sum / add, mean, min, max, var, std) of every row's messages: [M, len(aggrs), K]
     "spmm_multi": "(Tensor? row, Tensor rowptr, Tensor col, Tensor? value, Tensor? colptr, Tensor? csr2csc, "
                   "Tensor mat, Tensor? row_csc, str[] aggrs) -> Tensor",
+    # the softmax-weighted sum of every row's messages per column, with temperature t ([], [1] or [K]; None: 1)
+    "spmm_softmax_aggr": "(Tensor rowptr, Tensor col, Tensor? value, Tensor? colptr, Tensor? csr2csc, Tensor mat, "
+                         "Tensor? row_csc, Tensor? t) -> Tensor",
     # multi-head: value [E, H] over x [N, H, D]; scores [E, H] of a [M, H, D] and b [N, H, D]
     "spmm_heads": "(Tensor? row, Tensor rowptr, Tensor col, Tensor? value, Tensor? colptr, Tensor? csr2csc, "
                   "Tensor x, Tensor? row_csc) -> Tensor",
@@ -79,6 +83,7 @@ def _csr2csc(row, col, M: int, N: int):
 
 _EXTRA_IMPLS = {
     "spmm_sum_csc": ops.spmm_sum, "spmm_mean_csc": ops.spmm_mean, "spmm_res": ops.spmm_res, "spmm_multi": ops.spmm_multi,
+    "spmm_softmax_aggr": ops.spmm_softmax_aggr,
     "coalesce": ops.coalesce, "sort_perm": ops.sort_perm, "csr2csc": _csr2csc,
     "segment_reduce": lambda ptr, value, reduce, perm, seg: ops.segment_reduce(ptr, value, reduce, perm, seg),
     "spspmm": ops.spspmm,
